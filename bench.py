@@ -1,4 +1,4 @@
-"""FoV-steps/s and segmented-voxels/s benchmark of the B200 flood-fill engine (contract: DESIGN.md "Measurement").
+"""FoV-steps/s and segmented-voxels/s benchmark of the H100 flood-fill engine (contract: DESIGN.md "Measurement").
 
   python bench.py --gpus 1 --steps K --warmup W            # our arm, N = 1
   python bench.py --impl reference --steps K --warmup W    # reference arm (CPU restatement, rank 0 only)
@@ -10,13 +10,16 @@ Workloads (BASELINE.json):
           `run_inference.py configs/inference_training_sample2.pbtxt` on a 250^3 bounding box, i.e.
           Canvas.segment_all with PolicyPeaks seeds and the pbtxt's inference options, ConvStack3DFFNModel depth 12,
           fov 33^3, deltas 8, FIB-25 weights, on the synthetic stand-in for training_sample2 (Voronoi phantom,
-          seed 0; SURVEY.md 8d).  ONE timed pass = the whole canvas (~25.6 k FoV steps, ~585 objects): a flood
-          fill has no meaningful K-step prefix (seed policy, object commits and the last objects are part of
-          the metric), so --steps is IGNORED for sizing (profiler runs cap the seed list with --max-seeds);
-          `steps` in the output line is the number of FoV steps done.
+          seed 0; SURVEY.md 8d).  ONE timed step = one pass over the whole canvas (~25.6 k FoV steps, ~585
+          objects): a flood fill has no meaningful prefix (seed policy, object commits and the last objects are
+          part of the metric), so --steps K runs K such passes, each on a fresh canvas of the same volume
+          (profiler runs cap the seed list with --max-seeds); `fov_steps` in the output line is the number of FoV
+          steps done in them.
           `value` = FoV steps / wall clock of segment_all (device PolicyPeaks included) with the volume resident
           in HBM; `e2e` = the same metric through Runner.run (volume file -> pinned H2D -> segment_all -> D2H ->
           seg-*.npz / .prob written), which is what a user of run_inference.py gets.
+          --dump-outputs DIR writes what the last timed pass returned (dump_outputs) for output-by-output
+          comparisons of two builds.
   N > 1   configs[3] — a 1024^3 volume as 8 slabs of 512^3 (2x2x2), slabs_of_rank(8, rank, N) per GPU, every slab an
           independent canvas (the reference's subvolume semantics, doc/manual.md:107-127), then the merge inside the
           timed region: all_gather of the id counts, id offsets on the device, NCCL gather of the label AND
@@ -70,7 +73,8 @@ def load_weights():
 
 def make_volume(shape, seed):
   from ffn_b200.synthetic import voronoi_phantom
-  cache = os.path.join(os.environ.get('FFN_BENCH_CACHE', '/tmp/ffn_bench_cache'), 'vol_%d_%d.npy' % (shape[0], seed))
+  cache = os.path.join(os.environ.get('FFN_BENCH_CACHE', os.path.join(tempfile.gettempdir(), 'ffn_bench_cache')),
+                       'vol_%d_%d.npy' % (shape[0], seed))
   if os.path.exists(cache):
     return np.load(cache)
   vol = voronoi_phantom(shape, seed)
@@ -83,11 +87,12 @@ def make_volume(shape, seed):
 
 
 class ClockSampler:
-  """Samples nvidia-smi clocks / throttle reasons while the timed region runs."""
+  """Samples nvidia-smi clocks / throttle reasons while the timed region runs, and the card's name and power
+  limit, which belong with every number measured on it."""
 
   QUERY = ('clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,'
            'clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,'
-           'clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap')
+           'clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,name,power.limit')
 
   def __init__(self, index):
     self.index = index
@@ -120,12 +125,13 @@ class ClockSampler:
       return {'sm_mhz': None, 'sm_max_mhz': None, 'reasons': ['nvidia-smi unavailable']}
     time.sleep(0.15)
     self.proc.terminate()
-    sm, mx, reasons = [], [], set()
+    sm, mx, reasons, gpu, limit = [], [], set(), None, None
     names = ['hw_slowdown', 'hw_thermal_slowdown', 'sw_thermal_slowdown', 'sw_power_cap']
     for ln in self.lines:
       parts = [p.strip() for p in ln.split(',')]
-      if len(parts) < 8:
+      if len(parts) < 10:
         continue
+      gpu, limit = parts[8], parts[9]
       try:
         sm.append(float(parts[0])); mx.append(float(parts[1]))
       except ValueError:
@@ -134,33 +140,7 @@ class ClockSampler:
         if v.lower().startswith('active'):
           reasons.add(n)
     return {'sm_mhz': float(np.median(sm)) if sm else None, 'sm_max_mhz': max(mx) if mx else None,
-            'reasons': sorted(reasons), 'samples': len(sm)}
-
-
-def ncu_dram_traffic():
-  """DRAM bytes (read + write) per launch of the flood kernel from the newest committed `ncu --set full`
-  summary under profiles/ (file name carries the FoV steps of the captured launch), or None."""
-  import glob
-  import re
-  scale = {'byte': 1.0, 'Kbyte': 1e3, 'Mbyte': 1e6, 'Gbyte': 1e9}
-  for path in sorted(glob.glob(os.path.join(REPO, 'profiles', 'r*_ncu_full_flood_kernel_steps*.txt')), reverse=True):
-    m = re.search(r'steps(\d+)', os.path.basename(path))
-    total, seen = 0.0, 0
-    try:
-      with open(path) as f:
-        for line in f:
-          for key in ('dram__bytes_read.sum [', 'dram__bytes_write.sum ['):
-            if line.startswith(key):
-              unit = line[len(key):line.index(']')]
-              total += float(line.split('=')[1]) * scale[unit]
-              seen += 1
-    except (OSError, ValueError, KeyError):
-      continue
-    if seen == 2 and m:
-      n = int(m.group(1))
-      return {'bytes_per_launch': total, 'steps_per_launch': n, 'bytes_per_step': total / n,
-              'source': os.path.relpath(path, REPO)}
-  return None
+            'reasons': sorted(reasons), 'samples': len(sm), 'gpu': gpu, 'power_limit_w': limit}
 
 
 def measured_peaks():
@@ -168,8 +148,8 @@ def measured_peaks():
   if os.path.exists(path):
     with open(path) as f:
       d = json.load(f)
-    return d.get('bf16_tflops', 1590.0), d.get('bf16_tflops_sustained', 1400.0), 'measured (MEASURED_PEAKS.json)'
-  return 1590.0, 1400.0, 'fallback (B200_PROFILING.md)'
+    return d.get('bf16_tflops', 989.4), d.get('bf16_tflops_sustained', 989.4), 'measured (MEASURED_PEAKS.json)'
+  return 989.4, 989.4, 'H100 SXM data sheet, dense FP16 at 700 W (not a measured rate)'
 
 
 def best_cpu_threads():
@@ -268,7 +248,7 @@ def reference_arm(args, rank):
   if not n1:
     vol = vol[:256, :256, :256]     # bounded sample: a corner of slab 0 (the CPU seed policy alone is minutes on 512^3)
   threads = best_cpu_threads()
-  budget = args.steps if 0 < args.steps < 1000 else 24     # a bounded sample: ~1 s of CPU per FoV step on 8 cores
+  budget = args.steps if args.steps and 0 < args.steps < 1000 else 24     # a bounded sample: ~1 s of CPU per FoV step on 8 cores
   steps, vox, secs, t_seed = run_cpu_sample(vol, budget, threads)
   value = steps / secs
   line = {
@@ -354,6 +334,27 @@ def parity_fields(engine, eng, _lib):
   return out
 
 
+def dump_outputs(out_dir, canvas, seeds, origins, ctr, _lib):
+  """What the timed segment_all returned, as float arrays under out_dir: the labels and quantised probabilities at a
+  fixed sample of 2^20 voxels (RandomState(0), `sample_index` = flat C-order indices), the seed list, the origins
+  (id, z, y, x, FoV steps) and the counters except the timing ones."""
+  os.makedirs(out_dir, exist_ok=True)
+  seg = canvas.read(_lib.ARRAY_SEGMENTATION).ravel()
+  prob = canvas.read(_lib.ARRAY_QPROB).ravel()
+  idx = np.sort(np.random.RandomState(0).randint(0, seg.size, size=min(1 << 20, seg.size)))
+  arrays = {
+      'segmentation_sample': seg[idx].astype(np.float64),
+      'probability_sample': prob[idx].astype(np.float32),
+      'sample_index': idx.astype(np.float64),
+      'seeds': np.asarray(seeds, dtype=np.float64).reshape(-1, 3),
+      'origins': np.array([[o.id] + list(o.start_zyx) + [o.iters] for o in origins], dtype=np.float64).reshape(-1, 5),
+      'counters': np.array([getattr(ctr, n) for n, _ in _lib.Counters._fields_
+                            if n not in ('device_seconds', 'kernel_launches')], dtype=np.float64),
+  }
+  for name, a in arrays.items():
+    np.save(os.path.join(out_dir, name + '.npy'), a)
+
+
 def run_n1(args, rank, local_rank):
   import torch
   from ffn_b200 import _lib
@@ -376,31 +377,38 @@ def run_n1(args, rank, local_rank):
   warm.segment_all(wseeds[:max(8 * max(args.warmup, 3), 24)])
   warm.close()
 
-  # ---- device-resident leg: the volume is in HBM before the timed region starts
-  canvas = eng.DeviceCanvas(engine, pinned.numpy(), opts, 128.0, 33.0, keep_probability_maps=True)
+  # ---- device-resident leg, --steps timed passes: the volume is in HBM before each timed pass starts
   sampler = ClockSampler(local_rank)
   sampler.start()
   sampler.wait_ready()
-  torch.cuda.synchronize()
   launches0 = engine.info()['launches']
-  t0 = time.perf_counter()
-  seeds, _ = device_seeds(canvas)
-  t_seed = time.perf_counter() - t0
-  if seed_cap:
-    seeds = seeds[:seed_cap]
-  origins, _, ctr = canvas.segment_all(seeds, overlaps_cap=max(64 * len(seeds), 1 << 16))
-  torch.cuda.synchronize()
-  wall = time.perf_counter() - t0
+  wall = t_seed = dev_seconds = 0.0
+  steps = vox = executed = 0
+  for i in range(args.steps):
+    canvas = eng.DeviceCanvas(engine, pinned.numpy(), opts, 128.0, 33.0, keep_probability_maps=True)
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    seeds, _ = device_seeds(canvas)
+    t_seed += time.perf_counter() - t0
+    if seed_cap:
+      seeds = seeds[:seed_cap]
+    origins, _, ctr = canvas.segment_all(seeds, overlaps_cap=max(64 * len(seeds), 1 << 16))
+    torch.cuda.synchronize()
+    wall += time.perf_counter() - t0
+    spec = canvas.spec_stats()
+    steps += int(ctr.inference_calls)
+    vox += int(ctr.voxels_segmented)
+    dev_seconds += float(ctr.device_seconds)
+    executed += spec['steps_executed']
+    if args.dump_outputs and i == args.steps - 1:
+      dump_outputs(args.dump_outputs, canvas, seeds, origins, ctr, _lib)
+    canvas.close()
   clocks = sampler.stop()
-  launches = engine.info()['launches'] - launches0 + 10        # + the ten seed-policy kernels
-  spec = canvas.spec_stats()
-  steps = int(ctr.inference_calls)
-  dev_seconds = float(ctr.device_seconds)
-  canvas.close()
+  launches = engine.info()['launches'] - launches0 + 10 * args.steps       # + the ten seed-policy kernels per pass
 
   # ---- end-to-end leg: what run_inference.py does — Runner.start + Runner.run on a volume file
   if args.skip_e2e:
-    e2e_seconds, e2e_steps, e2e_vox = wall, steps, int(ctr.voxels_segmented)
+    e2e_seconds, e2e_steps, e2e_vox = wall, steps, vox
   else:
     from ffn.inference import runner as runner_mod
     tmp = tempfile.mkdtemp(prefix='ffn_bench_')
@@ -424,21 +432,21 @@ def run_n1(args, rank, local_rank):
   burst, sustained, src = measured_peaks()
   kernel_rate = steps / dev_seconds                                  # counted steps over the flood kernel's own time
   achieved = kernel_rate * flops_per_step() / 1e12
-  executed = spec['steps_executed'] / dev_seconds * flops_per_step() / 1e12
+  executed = executed / dev_seconds * flops_per_step() / 1e12
   line = {
       'metric': 'fov_steps_per_sec', 'value': value, 'unit': 'FoV steps/s', 'n_gpus': 1,
-      'steps': steps, 'warmup': max(args.warmup, 3), 'ms_per_step': 1e3 * wall / max(steps, 1),
+      'steps': args.steps, 'fov_steps': steps, 'warmup': max(args.warmup, 3), 'ms_per_step': 1e3 * wall / max(steps, 1),
       'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None,
       'dtype': {'fp16': 'f16', 'fp32': 'f32', 'x2': 'f16x2 (hi+lo split, ~f32)'}[args.compute], 'data': 'synthetic',
       'config': {
           'workload': WORKLOAD_N1,
-          'weights': wdesc, 'accumulate': 'f32', 'timed_pass': 'one whole segment_all (device PolicyPeaks + flood fill + commits); '
-          '--steps is ignored (a flood fill has no meaningful K-step prefix)' + (' — capped at %d seeds' % seed_cap if seed_cap else ''),
+          'weights': wdesc, 'accumulate': 'f32', 'timed_pass': 'one whole segment_all (device PolicyPeaks + flood fill + commits) '
+          'per step; ms_per_step is per FoV step' + (' — capped at %d seeds' % seed_cap if seed_cap else ''),
           'l2': 'canvas state (image u8 + 4 seed f32 arrays + segmentation i32 + qprob u8 = 330 MB) exceeds L2; '
-                'the ~25 MB activation working set of four chains is L2-resident by design',
+                'the step workspace of four chains (fp16 activations, fp32 residual stream) is ~45 MB against 50 MB of L2',
           'published_reference_p100': {'fov_steps_per_sec': 65.5, 'voxels_per_sec': 35216},
       },
-      'voxels_per_sec': float(ctr.voxels_segmented) / wall,
+      'voxels_per_sec': vox / wall,
       'segments': int(ctr.segments), 'objects_run': int(ctr.segment_at_calls), 'seeds': int(len(seeds)),
       'seed_policy_seconds': t_seed,
       'device_only': {'value': kernel_rate, 'unit': 'FoV steps/s', 'seconds': dev_seconds,
@@ -456,8 +464,7 @@ def run_n1(args, rank, local_rank):
                    'frac': achieved / burst, 'frac_of_sustained': achieved / sustained, 'peak_source': src,
                    'flops_per_step': flops_per_step(), 'executed_frac': executed / burst,
                    'note': 'achieved = counted FoV steps x FLOP/step / flood-kernel seconds (CUDA events around its '
-                           'launches); executed_frac also counts the steps of discarded early runs',
-                   'traffic': ncu_dram_traffic()},
+                           'launches); executed_frac also counts the steps of discarded early runs'},
   }
   if not args.skip_extras and args.compute == 'fp16':
     try:
@@ -623,8 +630,7 @@ def run_multi(args, rank, local_rank, world):
                         'segment_all, merged labels / probabilities left in rank 0 HBM (NCCL gather, no D2H)'},
         'roofline': {'bound': 'tensor', 'achieved': achieved, 'peak': burst, 'unit': 'TFLOP/s', 'frac': achieved / burst,
                      'frac_of_sustained': achieved / sustained, 'peak_source': src, 'flops_per_step': flops_per_step(),
-                     'note': 'per GPU: counted steps x FLOP/step / (busiest rank flood-kernel seconds x N)',
-                     'traffic': ncu_dram_traffic()},
+                     'note': 'per GPU: counted steps x FLOP/step / (busiest rank flood-kernel seconds x N)'},
     }
     print(json.dumps(line), flush=True)
   for cv, _ in canvases:
@@ -635,7 +641,7 @@ def run_multi(args, rank, local_rank, world):
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--gpus', type=int, default=1)
-  ap.add_argument('--steps', type=int, default=0)
+  ap.add_argument('--steps', type=int, default=None, help='N = 1: timed passes over the whole canvas (default 1)')
   ap.add_argument('--warmup', type=int, default=3)
   ap.add_argument('--impl', default='b200', choices=['b200', 'reference'])
   ap.add_argument('--compute', default='fp16', choices=['fp16', 'fp32', 'x2'])
@@ -646,7 +652,12 @@ def main():
   ap.add_argument('--cpu-baseline-steps', type=int, default=24)
   ap.add_argument('--skip-extras', action='store_true', help='no single-seed / predict / cpu_baseline legs (profiler runs)')
   ap.add_argument('--skip-e2e', action='store_true', help='no Runner.run leg (profiler runs; the line then repeats the device-resident value)')
+  ap.add_argument('--dump-outputs', metavar='DIR', help='N = 1: write what the last timed pass computed to DIR/<name>.npy')
   args = ap.parse_args()
+  if args.impl != 'reference':
+    args.steps = 1 if args.steps is None else args.steps
+    if args.steps < 1:
+      ap.error('--steps must be at least 1')
   rank = int(os.environ.get('RANK', '0'))
   local_rank = int(os.environ.get('LOCAL_RANK', '0'))
   world = int(os.environ.get('WORLD_SIZE', '1'))

@@ -91,7 +91,7 @@ def load() -> C.CDLL:
       build_if_needed()
     except Exception as e:  # pylint: disable=broad-except
       raise ImportError(
-          'libffn_b200.so is missing and could not be built (%s). The FFN B200 engine has no CPU '
+          'libffn_b200.so is missing and could not be built (%s). The FFN engine has no CPU '
           'fallback.' % e) from e
   lib = C.CDLL(LIB_PATH)
   p = C.c_void_p

@@ -1,4 +1,4 @@
-"""Builds libffn_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Builds libffn_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
 
 import os
 import subprocess
@@ -33,7 +33,7 @@ def build(force=False, verbose=False, defines=(), out=None):
     return OUT
   tmp = out + '.tmp%d' % os.getpid()   # linked next to the target and renamed over it: a reader never sees a partial file
   cmd = [
-      nvcc_path(), '-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17', '--default-stream', 'per-thread',
+      nvcc_path(), '-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '--default-stream', 'per-thread',
       '-Xcompiler', '-fPIC', '-shared', '-o', tmp, SRC, '-lcudart',
   ] + ['-D%s' % d for d in defines]
   if verbose:

@@ -10,26 +10,20 @@
 
 namespace ffn {
 
-constexpr int kThreads = 352;     // warps 0-7: epilogue (2 channel halves x 4 TMEM lane quarters); warp 8: TMA producer; warp 9: UMMA issuer;
-                                  // warp 10: signals the chains' split-phase barriers (the release stays off the epilogue's path)
+constexpr int kThreads = 320;     // warps 0-7: two consumer warpgroups (wgmma + epilogue, 64 accumulator rows each); warp 8: TMA producer;
+                                  // warp 9: signals the chains' split-phase barriers (the release stays off the epilogue's path)
 constexpr int kLoadWarp = 8;
-constexpr int kMmaWarp = 9;
-constexpr int kSigWarp = 10;
+constexpr int kSigWarp = 9;
 #ifndef FFN_ACT_STAGES
 #define FFN_ACT_STAGES 3
 #endif
 constexpr int kActStages = FFN_ACT_STAGES;     // shared-memory ring of per-tile activation operands
-#ifndef FFN_ACC_SLOTS
-#define FFN_ACC_SLOTS 2
-#endif
-constexpr int kAccSlots = FFN_ACC_SLOTS;      // TMEM ring of per-tile accumulators (measured: 2 slots cost nothing against 3 — the tile loads
-                                              // and the UMMA issue pace the pipeline — and leave TMEM columns for a fourth chain's residual)
-constexpr int kTileM = 128;       // UMMA M: accumulator rows per tensor-core tile
+constexpr int kTileM = 128;       // accumulator rows per tensor-core tile (two m64 warpgroup MMAs)
 constexpr int kTileOut = 126;     // FoV rows a tile OUTPUTS: the dx = -1/+1 partial sums live one row up/down, so
                                   // the first and last accumulator row of every tile only feed their neighbours
-constexpr int kStackN = 96;       // UMMA N: the three dx taps of a (dz, dy) tap-row stacked along N
-constexpr int kFeat = 32;         // feature maps of every hidden layer (UMMA N)
-constexpr int kGroupTiles = kAccSlots;    // accumulator slots in TMEM (the residual stream starts behind them)
+constexpr int kStackN = 96;       // MMA N: the three dx taps of a (dz, dy) tap-row stacked along N
+constexpr int kFeat = 32;         // feature maps of every hidden layer
+constexpr int kAccRegs = 64 * kStackN / 128;   // fp32 accumulators per consumer thread (m64n96 fragment)
 constexpr int kMaxConv = 32;      // 2 * depth limit
 #ifndef FFN_MAX_CHAINS
 #define FFN_MAX_CHAINS 4
@@ -42,9 +36,8 @@ constexpr int kBufsPerChain = FFN_BUFS_PER_CHAIN;  // object buffers per chain: 
 constexpr int kMaxBufs = kMaxChains * kBufsPerChain;
 constexpr int kSplitShift = 10;   // FFN_COMPUTE_FP16X2_TC: weights are split as w * 2^10 = hi + lo (keeps lo a normal fp16
                                   // number for |w| down to ~1e-4); the epilogue scales the accumulators back (exact)
-constexpr int kTmemCols = 512;    // accumulators (kGroupTiles * kStackN columns) + fp32 residual stream (32 per tile)
-constexpr int kMaxTilesPerCta = (kTmemCols - kGroupTiles * kStackN) / kFeat;   // 7 (3 slots) / 10 (2 slots): bound by the TMEM-resident residual
-static_assert(kAccSlots >= 2 && kAccSlots <= 3 && kMaxChains >= 1 && kMaxChains <= 5, "chains / accumulator slots");
+constexpr int kMaxTilesPerCta = 0xFFFF / kTileOut;   // the per-CTA step counts are packed into 16 bits (publish_counts)
+static_assert(kMaxChains >= 1 && kMaxChains <= 5, "chains");
 
 // Field-of-view geometry in the "row" space the kernels work in.
 //
@@ -53,7 +46,7 @@ static_assert(kAccSlots >= 2 && kAccSlots <= 3 && kMaxChains >= 1 && kMaxChains 
 // (dz halos are the zero guard rows before / after the FoV), so a (dz, dy) tap-row is the constant
 // row offset dz*pp + dy*xp.  The dx taps need no padding in memory: the tensor-core path stacks them
 // along N and adds the neighbouring rows' partial sums in the epilogue (skipping x = 0 / x = fx-1),
-// the fp32 path masks them.  Rows are cut into tiles of kTileOut output rows = one 128-row UMMA.
+// the fp32 path masks them.  Rows are cut into tiles of kTileOut output rows = one 128-row MMA tile.
 struct Geom {
   int fz, fy, fx;   // FoV size (z, y, x)
   int mz, my, mx;   // margin = size // 2
@@ -70,7 +63,7 @@ struct Geom {
 };
 
 struct Weights {
-  const __half* w16;   // per layer [9 tap-rows][kchunk][12 n-groups][8 n][8 k] fp16 (UMMA K-major, no swizzle),
+  const __half* w16;   // per layer [9 tap-rows][kchunk][12 n-groups][8 n][8 k] fp16 (wgmma K-major, no swizzle),
                        // n = dx * 32 + cout
   const __half* w16x2; // FFN_COMPUTE_FP16X2_TC: per layer the same packing twice, [hi | lo] parts of w * 2^kSplitShift
   const float* w32;    // per layer [27][cin_padded][32] fp32
@@ -132,6 +125,7 @@ struct ChainDev {
   float* logits;              // [nt*128] network output (seed + update), before the disco merge
   unsigned* count;            // [2 round parities][2]: voxels with logit >= move threshold; Canvas.history_deleted
   unsigned* bar;              // split-phase barrier of this chain: arrivals of the epilogue groups
+  float* res;                 // [nt*128][32] fp32 residual stream of the tensor-core modes, in consumer-thread order (tc_epilogue)
 };
 
 enum Phase : int {
@@ -284,12 +278,12 @@ struct KParams {
 };
 
 // The small-structures area at SmemLayout::bars (byte offsets from there):
-//   [0, 160)        mbarriers + the TMEM base address
+//   [0, 160)        mbarriers
 //   kOffMisc        s_misc: ints [0, kMaxChains) per-chain step-count accumulators, [7] abort flag copy,
 //                   [8, 8 + kMaxChains) disco flags, [16 + 32 k ...) movement-policy scratch of chain k
 //   kOffRound       s_round: [2 * kMaxChains][8] ints
 //   kOffProf        16 cycle counters (profiled build)
-//   kOffXchg        epilogue exchange (2 KB) + conv_lom dots (1 KB).  The leader's working copies of the chain states
+//   kOffXchg        epilogue exchange (4 KB).  The leader's working copies of the chain states
 //                   (kStateSlot bytes each) and of the scheduler block ALIAS this region: CTA 0 uses them only between
 //                   the grid barrier and the end of leader_round, when no epilogue is running.
 constexpr int kStateSlot = 352;
@@ -298,7 +292,7 @@ constexpr int kMiscAbort = 7, kMiscDisco = 8, kMiscScratch = 16;
 constexpr int kOffRound = kOffMisc + (kMiscScratch + 32 * kMaxChains) * 4;
 constexpr int kOffProf = kOffRound + 2 * kMaxChains * 8 * 4;
 constexpr int kOffXchg = (kOffProf + 16 * 8 + 15) / 16 * 16;
-constexpr int kXchgBytes = 2 * 2 * 4 * 2 * 16 * 4 + 2 * 128 * 4;   // s_xchg + s_dot
+constexpr int kXchgBytes = 2 * 8 * 2 * 4 * 8 * 4;   // s_xchg: [2 tile parities][8 warps][2 directions][4 lanes][8]
 constexpr int kBarsAreaBytes = kOffXchg + kXchgBytes;
 
 // Shared-memory carve-up (bytes from the 1024-aligned base).

@@ -155,11 +155,8 @@ Geom make_geom(const FfnModelDesc& m) {
   return g;
 }
 
-// How many chains a launch may use: the fp32 residual stream of every (chain, tile) lives in TMEM.
-int chain_limit(const FfnEngine* e) {
-  const int tiles = (e->g.nt + e->grid - 1) / e->grid;
-  return std::max(1, std::min({e->max_chains, (int)kMaxChains, kMaxTilesPerCta / std::max(tiles, 1)}));
-}
+// How many chains a launch may use.
+int chain_limit(const FfnEngine* e) { return std::max(1, std::min(e->max_chains, (int)kMaxChains)); }
 
 // Launches the persistent kernel once and waits for it.  `c` may be null (predict).
 int launch(FfnEngine* e, FfnCanvas* c, int nchains, const Job& job) {
@@ -380,9 +377,9 @@ int ffn_engine_create(int device, const FfnModelDesc* model, const float* const*
   if (device < 0 || device >= ndev) return fail("bad device index");
   cudaDeviceProp prop{};
   CUDA_OK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10)
+  if (prop.major != 9 || prop.minor != 0)
     return fail(std::string("device is sm_") + std::to_string(prop.major) + std::to_string(prop.minor) +
-                "; this library only contains sm_100a code");
+                "; this library only contains sm_90a code");
   std::unique_ptr<FfnEngine> e(new FfnEngine());
   e->device = device;
   CUDA_OK(cudaSetDevice(device));
@@ -413,8 +410,7 @@ int ffn_engine_create(int device, const FfnModelDesc* model, const float* const*
   if (per_sm < 1) return fail("persistent kernel does not fit on an SM");
   e->grid = std::min(e->sm_count, g.nt);
   if ((g.nt + e->grid - 1) / e->grid > kMaxTilesPerCta)
-    return fail("field of view needs more than " + std::to_string(kMaxTilesPerCta) +
-                " tiles per SM: the TMEM-resident residual stream does not fit (too few SMs for this FoV)");
+    return fail("field of view needs more than " + std::to_string(kMaxTilesPerCta) + " tiles per SM");
 
   // weights
   std::vector<__half> w16, w16x2;
@@ -459,8 +455,8 @@ int ffn_engine_create(int device, const FfnModelDesc* model, const float* const*
   for (void* p : std::vector<void*>{ws.act0_l, ws.act_l[0], ws.act_l[1], ws.act0_f, ws.act_f[0], ws.act_f[1], ws.res,
                                     ws.bar, ws.abort_flag, ws.prof})
     e->owned.push_back(p);
-  for (int k = 0; k < kMaxChains; ++k) {   // per-chain step workspace: fp16 operands, raw seed, logits, counters, barrier
-    ChainDev& cw = e->cws[k];
+  for (int k = 0; k < kMaxChains; ++k) {   // per-chain step workspace: fp16 operands, raw seed, logits, counters, barrier,
+    ChainDev& cw = e->cws[k];              // fp32 residual stream
     if (dev_alloc(&cw.act0_h, 2 * ra * 8)) return 1;
     if (dev_alloc(&cw.act_h[0], 4 * ra * 8)) return 1;
     if (dev_alloc(&cw.act_h[1], 4 * ra * 8)) return 1;
@@ -469,8 +465,9 @@ int ffn_engine_create(int device, const FfnModelDesc* model, const float* const*
     if (dev_alloc(&cw.logits, (size_t)g.nt * kTileM)) return 1;
     if (dev_alloc(&cw.count, 4)) return 1;
     if (dev_alloc(&cw.bar, 1)) return 1;
+    if (dev_alloc(&cw.res, (size_t)g.nt * kTileM * kFeat)) return 1;
     for (void* p : std::vector<void*>{cw.act0_h, cw.act_h[0], cw.act_h[1], cw.seed_raw[0], cw.seed_raw[1], cw.logits,
-                                      cw.count, cw.bar})
+                                      cw.count, cw.bar, cw.res})
       e->owned.push_back(p);
   }
   // Tensor maps for the tile loads (driver entry point fetched at run time: no link-time dependency on libcuda).
@@ -495,10 +492,8 @@ int ffn_engine_create(int device, const FfnModelDesc* model, const float* const*
                                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
                                             CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
       }
-    // Measured (B200, round 2): the tiled copy moves this layout as 16-byte rows (the k-chunk is the innermost
-    // extent) and needs 2.5x longer per tile than the twelve 3 KB 1-D bulk copies (UBLKCP, the same TMA engine):
-    // 13.1 k vs 16.8 k patches/s in ffn_predict(batch=48).  The bulk path is therefore the default;
-    // FFN_B200_TMAP=1 selects the tensor-map path.
+    // The tiled copy moves this layout as 16-byte rows (the k-chunk is the innermost extent), so the twelve 1-D
+    // bulk copies per tile are the default; FFN_B200_TMAP=1 selects the tensor-map path.
     const char* env = std::getenv("FFN_B200_TMAP");
     e->use_tmap = (ok && env && std::atoi(env) != 0) ? 1 : 0;
   }
@@ -525,7 +520,7 @@ int ffn_engine_set_grid(FfnEngine* e, int num_ctas) {
   if (num_ctas <= 0) num_ctas = std::min(e->sm_count, e->g.nt);
   if (num_ctas > e->sm_count || num_ctas > e->g.nt) return fail("grid larger than the SM / tile count");
   if ((e->g.nt + num_ctas - 1) / num_ctas > kMaxTilesPerCta)
-    return fail("grid too small: at most " + std::to_string(kMaxTilesPerCta) + " tiles per CTA (TMEM residual)");
+    return fail("grid too small: at most " + std::to_string(kMaxTilesPerCta) + " tiles per CTA");
   e->grid = num_ctas;
   return 0;
 }

@@ -2,7 +2,7 @@
 //
 // ONE cooperative launch runs whole objects (or a whole canvas): per FoV step it stages the
 // (image, seed) tile from the HBM-resident canvas, evaluates the residual conv stack with the
-// field of view spread over all CTAs (tcgen05 implicit GEMM, or fp32 FMA in the parity mode),
+// field of view spread over all CTAs (wgmma implicit GEMM, or fp32 FMA in the parity mode),
 // fuses bias / ReLU / residual / conv_lom / seed-add as epilogues, applies the disco merge,
 // pastes into the seed canvas, evaluates the face-max movement policy and pops the next position
 // from the device-side queue — without returning to the host.
@@ -10,7 +10,7 @@
 // Up to kMaxChains flood fills ("chains": independent objects of one canvas, or independent patches of a
 // batched predict) are TIME-MULTIPLEXED over all SMs: the kernel works in rounds, a round runs one FoV step
 // of every active chain, and inside a round the layers of the chains are interleaved — (layer 0: chain A, B,
-// C), (layer 1: A, B, C), ... — through one TMA -> UMMA -> epilogue pipeline per CTA.  The dependency
+// C), (layer 1: A, B, C), ... — through one TMA -> wgmma + epilogue pipeline per CTA.  The dependency
 // "layer l of chain A needs layer l-1 of chain A from EVERY CTA" is a split-phase barrier per chain: the
 // epilogue warps arrive (red.release) and move on to the next chain's tile, only the TMA producer waits
 // (ld.acquire) just before it loads that chain's operands.  The barrier / L2 latency of one chain is thereby
@@ -33,7 +33,7 @@
 #include <math_constants.h>
 
 #include "device_types.cuh"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace ffn {
 namespace FFN_KNS {
@@ -52,17 +52,13 @@ struct Ctx {
   unsigned char* smem;
   float* s_bias;               // [(nconv)*32] biases, then w_lom[32], b_lom
   uint64_t* mb_w;              // [2]
-  uint64_t* mb_full;           // [kActStages] TMA -> UMMA: a tile's operands have landed
-  uint64_t* mb_empty;          // [kActStages] UMMA -> TMA: the stage may be overwritten
-  uint64_t* mb_tfull;          // [kAccSlots]  UMMA -> epilogue: accumulators complete
-  uint64_t* mb_tempty;         // [kAccSlots]  epilogue -> UMMA: accumulators drained (8 arrivals)
+  uint64_t* mb_full;           // [kActStages] TMA -> consumers: a tile's operands have landed
+  uint64_t* mb_empty;          // [kActStages] consumers -> TMA: the stage may be overwritten (8 arrivals)
   uint64_t* mb_sig;            // [kMaxChains] epilogue -> signal warp: a chain's layer is stored (8 arrivals)
-  unsigned load_cnt, mma_cnt, epi_cnt;   // per-role running tile counters (ring index + phase parity)
-  uint32_t* s_tmem;            // TMEM base address
+  unsigned load_cnt, epi_cnt;  // per-role running tile counters (ring index + phase parity)
   int* s_misc;                 // per-chain step-count accumulators, abort copy, disco flags, leader scratch (device_types.cuh: kOffMisc)
   int* s_round;                // [k][8] this round: action, z, y, x, buffer ; [kMaxChains + k][8] previous step: flags, z, y, x, buffer
-  float* s_xchg;               // [2 tile parities][2 halves][4 warps][2][16] partial sums crossing warp boundaries
-  float* s_dot;                // [2][128] conv_lom partial dot products of the upper channel half
+  float* s_xchg;               // [2 tile parities][8 warps][2 directions][4 lanes][8] partial sums crossing warp boundaries
   CanvasState* s_state;        // CTA 0: shared-memory working copies of the chain states (512-byte slots)
   Sched* s_sched;              // CTA 0: working copy of the scheduler state
   long long* prof;             // profiling slots of this CTA in SHARED memory (null unless CTA 0 / G-1);
@@ -74,7 +70,6 @@ struct Ctx {
   // mbarrier phase parities and pending-prefetch flags as ONE bit field: dynamically indexed arrays
   // would push this whole struct into local memory (behind the L1 every grid barrier invalidates).
   uint32_t bits;   // bit b: weights[b] parity; 8+b: weights[b] in flight
-  uint32_t tmem_base;
 };
 
 __device__ __forceinline__ uint32_t bit_get(const Ctx& c, int k) { return (c.bits >> k) & 1u; }
@@ -96,7 +91,7 @@ __device__ __forceinline__ CanvasState* chain_state(const Ctx& c, int k) {
 }
 
 __device__ __forceinline__ bool aborted(const Ctx& c) {
-  return sm100::ld_volatile_s32(c.p->ws.abort_flag) != 0;
+  return sm90::ld_volatile_s32(c.p->ws.abort_flag) != 0;
 }
 
 // Profiling is opt-in (ffn_engine_profile_enable): reading the clock is not free, and CTA G-1 —
@@ -107,8 +102,8 @@ __device__ __forceinline__ void prof_add(const Ctx& c, int slot, long long dt) {
   if (c.prof) c.prof[slot] += dt;
 }
 // Tile timeline of one CTA (ffn_engine_trace): event e of the role's idx-th tile since kernel start.
-//   0 producer saw the chain barrier   1 tile's copies issued   2 UMMA issuer saw the operands   3 ... got a TMEM slot
-//   4 UMMAs issued   5 epilogue saw the accumulators   6 epilogue done   7 signaller released (idx = signal number)
+//   0 producer saw the chain barrier   1 tile's copies issued   2 consumers saw the operands   4 MMAs complete
+//   6 epilogue done   7 signaller released (idx = signal number)
 __device__ __forceinline__ void trace_ev(const Ctx& c, int ev, unsigned idx) {
   if (c.trace && idx < (unsigned)kTraceTiles) c.trace[ev * kTraceTiles + idx] = clock64();
 }
@@ -122,7 +117,7 @@ __device__ __forceinline__ void trace_ev(const Ctx&, int, unsigned) {}
 __device__ __forceinline__ void mbar_wait(const Ctx& c, uint64_t* bar, uint32_t parity) {
   unsigned spins = 0;
   long long t0 = 0;
-  while (!sm100::mbar_try_wait(bar, parity)) {
+  while (!sm90::mbar_try_wait(bar, parity)) {
     if ((++spins & 0x3FF) == 0) {
       if (aborted(c)) return;
       const long long now = clock64();
@@ -139,7 +134,7 @@ __device__ __forceinline__ void mbar_wait(const Ctx& c, uint64_t* bar, uint32_t 
 __device__ __forceinline__ void spin_until(const Ctx& c, const unsigned* ctr, unsigned target, int code) {
   long long tw = 0;
   unsigned spins = 0;
-  while ((int)(sm100::ld_acquire_u32(ctr) - target) < 0) {
+  while ((int)(sm90::ld_acquire_u32(ctr) - target) < 0) {
     if ((++spins & 0xFF) == 0) {
       if (aborted(c)) break;
       const long long now = clock64();
@@ -156,7 +151,6 @@ __device__ __forceinline__ void spin_until(const Ctx& c, const unsigned* ctr, un
 // One red.release per CTA counts the arrival; one thread polls with acquire loads and releases the
 // others through a named barrier.
 __device__ __forceinline__ void grid_barrier(Ctx& c) {
-  sm100::tc_fence_before();
   __syncthreads();
   c.bar_target += c.G;
   if (c.warp == kLoadWarp) {
@@ -164,7 +158,7 @@ __device__ __forceinline__ void grid_barrier(Ctx& c) {
       const long long t0 = prof_now(c);
       // release: everything this CTA wrote (ordered before by bar.sync) becomes visible gpu-wide
       // before the arrival is counted
-      sm100::red_release_add(c.p->ws.bar, 1u);
+      sm90::red_release_add(c.p->ws.bar, 1u);
       spin_until(c, c.p->ws.bar, c.bar_target, 1);
       // the acquire load that observed the full count orders every later read of this CTA (after
       // the named barrier below) behind the other CTAs' writes; TMA readers add their proxy fence
@@ -176,7 +170,6 @@ __device__ __forceinline__ void grid_barrier(Ctx& c) {
   } else {
     asm volatile("bar.sync 4, %0;" ::"n"(kThreads) : "memory");
   }
-  sm100::tc_fence_after();
 }
 
 // Split-phase barrier of one chain.  ARRIVE: each of the eight epilogue warps, after its global stores of one
@@ -186,13 +179,12 @@ __device__ __forceinline__ void grid_barrier(Ctx& c) {
 // layer).  WAIT (the TMA producer warp, before it loads chain k's operands of the next layer): acquire-poll
 // until `events` arrivals of every CTA have been counted since the start of this chain's round.
 __device__ __forceinline__ void chain_arrive_epi(Ctx& c, int k) {
-  sm100::tc_fence_before();
   __syncwarp();
-  if (c.lane == 0) sm100::mbar_arrive(&c.mb_sig[k]);   // release.cta: this warp's stores -> the signal warp
+  if (c.lane == 0) sm90::mbar_arrive(&c.mb_sig[k]);   // release.cta: this warp's stores -> the signal warp
 }
 __device__ __forceinline__ void chain_signal(Ctx& c, int k, uint32_t parity) {   // signal warp
   mbar_wait(c, &c.mb_sig[k], parity);                     // acquire.cta: the eight epilogue warps' stores
-  if (c.lane == 0) sm100::red_release_add(c.p->ch[k].bar, 1u);   // cumulative: they become visible gpu-wide first
+  if (c.lane == 0) sm90::red_release_add(c.p->ch[k].bar, 1u);   // cumulative: they become visible gpu-wide first
   __syncwarp();
 }
 __device__ __forceinline__ void chain_wait(Ctx& c, int k, unsigned events) {
@@ -368,25 +360,25 @@ __device__ __forceinline__ void epilogue_row(const Ctx& c, int layer, int r, flo
 // ------------------------------------------------------------------------------------------
 // Tensor-core layer: implicit GEMM, M = 128 FoV rows, N = 32 features, K = 27 taps x Cin.
 // A = activation rows (K-major, no swizzle: [k-chunk][row] 16-byte units, so a tap is a shifted
-// start address), B = packed weights, D = fp32 accumulators in TMEM (32 columns per tile).
+// start address), B = packed weights, D = fp32 accumulators in the registers of the two consumer
+// warpgroups (rows 0-63 / 64-127 of the tile).
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ void tc_issue_weight_load(Ctx& c, int layer) {
   const KParams& p = *c.p;
   const int buf = layer & 1;
   const uint32_t bytes = (layer == 0 ? 27 * 2 : 27 * 4) * 512;
-  sm100::mbar_expect_tx(&c.mb_w[buf], bytes);
-  sm100::bulk_g2s(c.smem + buf * (27 * 4 * 512), p.w.w16 + w16_layer_offset_halfs(layer), bytes, &c.mb_w[buf]);
+  sm90::mbar_expect_tx(&c.mb_w[buf], bytes);
+  sm90::bulk_g2s(c.smem + buf * (27 * 4 * 512), p.w.w16 + w16_layer_offset_halfs(layer), bytes, &c.mb_w[buf]);
 }
 
-// Issues the 9 * NCH/2 UMMAs (128 x 96 x 16) of one tile: one per (dz, dy) tap-row and k-pair; the
-// three dx taps ride along N.  Fully unrolled: every A start-address offset is
-// (const * seg_rows + const * xp), so the loop body is two adds and the UMMA.
+// This warpgroup's 64 accumulator rows of one tile: 9 * NCH/2 MMAs 64 x 96 x 16, one per (dz, dy) tap-row
+// and k-pair; the three dx taps ride along N.  `a_lo` / `b_lo` are the low descriptor words (start address,
+// LBO) of the warpgroup's first A row in the stage and of the layer's weights; every A start-address offset is
+// (const * seg_rows + const * xp).  Returns when the MMAs have completed (the stage may be released).
 template <int NCH>
-__device__ __forceinline__ void tc_issue_tile(uint32_t d, uint32_t a_lo, uint32_t b_lo, int seg_rows, int xp) {
-  const uint32_t idesc = sm100::umma_idesc_f16(kTileM, kStackN);
-  const uint64_t hi = (uint64_t)((128u >> 4) | (1u << 14)) << 32;   // SBO = 128 B, descriptor version 1
-  // one (dz, dy) tap-row per iteration: fully unrolled, the 36 descriptors overflow the uniform register
-  // file into ordinary registers
+__device__ __forceinline__ void tc_mma_tile(float (&d)[kAccRegs], uint32_t a_lo, uint32_t b_lo, int seg_rows, int xp) {
+  const uint64_t hi = (uint64_t)(128u >> 4) << 32;   // SBO = 128 B
+  sm90::wgmma_fence();
 #pragma unroll 1
   for (int row = 0; row < 9; ++row) {
     const int tz = row / 3, ty = row % 3;
@@ -394,167 +386,164 @@ __device__ __forceinline__ void tc_issue_tile(uint32_t d, uint32_t a_lo, uint32_
     for (int j = 0; j < NCH / 2; ++j) {
       const uint32_t aoff = (uint32_t)((2 * j * 3 + tz) * seg_rows + ty * xp);   // stage layout [k-chunk][dz][row]
       const uint32_t boff = (uint32_t)((row * NCH + 2 * j) * (12 * 128 / 16));
-      sm100::umma_f16(d, hi | (uint64_t)(a_lo + aoff), hi | (uint64_t)(b_lo + boff), idesc,
-                      (row | j) != 0 ? 1u : 0u);
+      sm90::wgmma_m64n96k16(d, hi | (uint64_t)(a_lo + aoff), hi | (uint64_t)(b_lo + boff), (row | j) != 0 ? 1u : 0u);
     }
   }
+  sm90::wgmma_commit();
+  sm90::wgmma_wait_all();
 }
 
-__device__ __forceinline__ void quad_sync(int quad) {   // the four epilogue warps of one channel half
-  asm volatile("bar.sync %0, 128;" ::"r"(quad + 1) : "memory");
+// Split-fp16 form (FFN_COMPUTE_FP16X2_TC): stage layout [dz][k-chunk][row] for the hi parts at `aa_hi` and the lo
+// parts at `aa_lo`, weights w_hi / w_lo.  The tensor core truncates when it aligns an MMA's sum to the accumulator,
+// so the error of every accumulation scales with the accumulator's magnitude: the small cross terms (a_lo*w_hi,
+// a_hi*w_lo, ~2^-11 of the result) go in FIRST, while the accumulator is small, the 9*nch/2 main MMAs last.
+__device__ __forceinline__ void tc_mma_tile_x2(float (&d)[kAccRegs], uint32_t aa_hi, uint32_t aa_lo, uint32_t bw_hi,
+                                               uint32_t bw_lo, int nch, int seg_rows, int xp) {
+  const uint64_t hi = (uint64_t)(128u >> 4) << 32;
+  sm90::wgmma_fence();
+#pragma unroll 1
+  for (int pass = 0; pass < 2; ++pass) {
+#pragma unroll 1
+    for (int row = 0; row < 9; ++row) {
+      const int tz = row / 3, ty = row % 3;
+      for (int jj = 0; jj < nch / 2; ++jj) {
+        const uint32_t aoff = (uint32_t)((tz * nch + 2 * jj) * seg_rows + ty * xp);
+        const uint32_t boff = (uint32_t)((row * nch + 2 * jj) * (12 * 128 / 16));
+        if (pass == 0) {
+          sm90::wgmma_m64n96k16(d, hi | (uint64_t)(aa_lo + aoff), hi | (uint64_t)(bw_hi + boff), (row | jj) != 0 ? 1u : 0u);
+          sm90::wgmma_m64n96k16(d, hi | (uint64_t)(aa_hi + aoff), hi | (uint64_t)(bw_lo + boff), 1u);
+        } else {
+          sm90::wgmma_m64n96k16(d, hi | (uint64_t)(aa_hi + aoff), hi | (uint64_t)(bw_hi + boff), 1u);
+        }
+      }
+    }
+  }
+  sm90::wgmma_commit();
+  sm90::wgmma_wait_all();
 }
 
-// Epilogue of the tensor-core layer (warps 0-7; 2 channel halves x 4 TMEM lane quarters), specialised
-// by layer kind so that the residual / conv_lom paths cost nothing where they do not apply:
+// Epilogue of one tile (warps 0-7, straight from the accumulator registers), specialised by layer kind so that
+// the residual / conv_lom paths cost nothing where they do not apply:
 //   EPI_A        "_a" convolutions   : out = relu(v + b)                          (convstack_3d.py:38,45)
 //   EPI_B_FIRST  conv0_b             : net = v + b            ; out = relu(net)   (:39) starts the residual stream
 //   EPI_B        conv{i}_b, i >= 1   : net = v + b + residual ; out = relu(net)   (:46-49)
 //   EPI_LAST     the final "_b"      : as EPI_B, then logits = seed + b_lom + <relu(net), w_lom> (:51-54, model.py:176-177)
-// The fp32 residual stream lives in this thread's TMEM lane, columns behind the accumulator ring
-// (32 columns per tile and chain).
-// Accumulator row m of a tile holds, for the FoV row u = tile_row0 - 1 + m,
+// Thread (warp w, lane l) holds accumulator rows m = 16 w + l/4 and m + 8, and for each of them output channels
+// 8 i + 2 (l % 4) + e (i < 4, e < 2) of the three dx blocks.  Accumulator row m holds, for the FoV row
+// u = tile_row0 - 1 + m,
 //   D[u][dx*32 + co] = sum_{dz,dy,ci} act[u + dz*pp + dy*xp][ci] * W[dz,dy,dx][ci][co]
-// and the convolution output is out[v] = D[v-1][dx=-1] + D[v][dx=0] + D[v+1][dx=+1]: one lane up /
-// down, done with warp shuffles (+ a 2 KB shared-memory exchange at the three warp boundaries).
+// and the convolution output is out[v] = D[v-1][dx=-1] + D[v][dx=0] + D[v+1][dx=+1]: one row up / down, i.e. four
+// lanes up / down with warp shuffles, plus a shared-memory exchange at the warp boundaries.  The fp32 residual
+// stream of every (chain, tile) lives in global memory (L2), in this thread order, read and written by the same thread.
 enum EpiKind : int { EPI_A = 0, EPI_B_FIRST = 1, EPI_B = 2, EPI_LAST = 3 };
 
 template <int KIND, bool X2 = false>
-__device__ __forceinline__ int tc_epilogue(Ctx& c, int k, int layer, int ntiles) {
+__device__ __forceinline__ int tc_epilogue(Ctx& c, int k, int layer, int j, const float (&d)[kAccRegs]) {
   const KParams& p = *c.p;
   const Geom& g = p.g;
   const ChainDev& ch = p.ch[k];
   constexpr float kUnscale = 1.0f / (float)(1 << kSplitShift);   // X2: accumulators carry w * 2^kSplitShift
   constexpr bool kReadRes = KIND == EPI_B || KIND == EPI_LAST;
   constexpr bool kWriteRes = KIND == EPI_B_FIRST || KIND == EPI_B;
-  const int half = c.warp >> 2, wq = c.warp & 3;
-  const float4* bias4 = reinterpret_cast<const float4*>(c.s_bias + layer * 32 + half * 16);   // re-read per tile: 16 registers less
+  const int t = c.lane & 3, gq = c.lane >> 2;
+  const int tile = c.t_begin + j;
+  const int m0 = c.warp * 16 + gq;                     // accumulator rows of this thread: m0, m0 + 8
+  float* xch = c.s_xchg + (c.epi_cnt & 1) * (8 * 2 * 4 * 8);   // double-buffered by tile parity
+  // fragment index of (dx block b, row half h, channel slot q = 2 i + e): 4 * (4 b + i) + 2 h + e
+#define ACC(b, h, q) d[4 * (4 * (b) + ((q) >> 1)) + 2 * (h) + ((q) & 1)]
+  if (gq == 7) {   // row 15 of the dx = -1 block: consumed by row 0 of the next warp
+    float4* q4 = reinterpret_cast<float4*>(xch + ((c.warp * 2 + 0) * 4 + t) * 8);
+    q4[0] = make_float4(ACC(0, 1, 0), ACC(0, 1, 1), ACC(0, 1, 2), ACC(0, 1, 3));
+    q4[1] = make_float4(ACC(0, 1, 4), ACC(0, 1, 5), ACC(0, 1, 6), ACC(0, 1, 7));
+  }
+  if (gq == 0) {   // row 0 of the dx = +1 block: consumed by row 15 of the previous warp
+    float4* q4 = reinterpret_cast<float4*>(xch + ((c.warp * 2 + 1) * 4 + t) * 8);
+    q4[0] = make_float4(ACC(2, 0, 0), ACC(2, 0, 1), ACC(2, 0, 2), ACC(2, 0, 3));
+    q4[1] = make_float4(ACC(2, 0, 4), ACC(2, 0, 5), ACC(2, 0, 6), ACC(2, 0, 7));
+  }
+  asm volatile("bar.sync 3, 256;" ::: "memory");
+  // up[h][q] = D[m-1][dx=-1], dn[h][q] = D[m+1][dx=+1] for the rows m = m0 + 8 h
+  const int src_up = (c.lane + 28) & 31, src_dn = (c.lane + 4) & 31;
+  float up[2][8], dn[2][8];
+#pragma unroll
+  for (int q = 0; q < 8; ++q) {
+    const float xa = __shfl_sync(0xffffffffu, ACC(0, 0, q), src_up), xb = __shfl_sync(0xffffffffu, ACC(0, 1, q), src_up);
+    const float ya = __shfl_sync(0xffffffffu, ACC(2, 0, q), src_dn), yb = __shfl_sync(0xffffffffu, ACC(2, 1, q), src_dn);
+    up[0][q] = xa;                    // row m0 - 1 (gq = 0: previous warp, below)
+    up[1][q] = gq ? xb : xa;          // row m0 + 7
+    dn[0][q] = gq < 7 ? ya : yb;      // row m0 + 1
+    dn[1][q] = yb;                    // row m0 + 9 (gq = 7: next warp, below)
+  }
+  if (gq == 0 && c.warp > 0) {
+    const float4* q4 = reinterpret_cast<const float4*>(xch + (((c.warp - 1) * 2 + 0) * 4 + t) * 8);
+    const float4 u0 = q4[0], u1 = q4[1];
+    up[0][0] = u0.x; up[0][1] = u0.y; up[0][2] = u0.z; up[0][3] = u0.w;
+    up[0][4] = u1.x; up[0][5] = u1.y; up[0][6] = u1.z; up[0][7] = u1.w;
+  }
+  if (gq == 7 && c.warp < 7) {
+    const float4* q4 = reinterpret_cast<const float4*>(xch + (((c.warp + 1) * 2 + 1) * 4 + t) * 8);
+    const float4 u0 = q4[0], u1 = q4[1];
+    dn[1][0] = u0.x; dn[1][1] = u0.y; dn[1][2] = u0.z; dn[1][3] = u0.w;
+    dn[1][4] = u1.x; dn[1][5] = u1.y; dn[1][6] = u1.z; dn[1][7] = u1.w;
+  }
   const size_t chunk_stride = (size_t)g.rows_alloc * 8;
-  __half* out_base = ch.act_h[layer & 1] + (size_t)(half * 2) * chunk_stride + (size_t)g.guard * 8;
-  __half* out_lo_base = X2 ? p.ws.act_l[layer & 1] + (size_t)(half * 2) * chunk_stride + (size_t)g.guard * 8 : nullptr;
+  const float* bias = c.s_bias + layer * 32 + 2 * t;
   const float* raw_in = ch.seed_raw[c.round & 1u];
   int hit = 0;
-  for (int j = 0; j < ntiles; ++j) {
-    const int slot = c.epi_cnt % kAccSlots;
-    float* xch = c.s_xchg + ((c.epi_cnt & 1) * 2 + half) * (4 * 2 * 16);   // double-buffered by tile parity
-    const int m = wq * 32 + c.lane;                                 // accumulator row of this thread
-    const int r = (c.t_begin + j) * kTileOut - 1 + m;               // FoV row it holds partial sums for
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m = m0 + 8 * h;
+    const int r = tile * kTileOut - 1 + m;             // FoV row of accumulator row m
     int z = 0, y = 0, x = 1;
     const bool valid = m >= 1 && m <= kTileOut && r >= 0 && row_to_zyx(g, r, z, y, x);
-    long long t0 = prof_now(c);
-    mbar_wait(c, &c.mb_tfull[slot], (c.epi_cnt / kAccSlots) & 1u);
-    if (c.tid == 0) prof_add(c, 4, prof_now(c) - t0);
-    if (c.tid == 0) trace_ev(c, 5, c.epi_cnt);
-    t0 = prof_now(c);
-    sm100::tc_fence_after();
-    const uint32_t tbase = c.tmem_base + ((uint32_t)(wq * 32) << 16) + (uint32_t)(slot * kStackN + half * 16);
-    const uint32_t tres = c.tmem_base + ((uint32_t)(wq * 32) << 16) +
-                          (uint32_t)(kAccSlots * kStackN + (k * ntiles + j) * kFeat + half * 16);
-    uint32_t a[16], b[16], d2[16], rr[16];
-    sm100::tmem_ld16(tbase, a);          // dx = -1 block: consumed by the lane above (m + 1)
-    sm100::tmem_ld16(tbase + 32, b);     // dx =  0 block
-    sm100::tmem_ld16(tbase + 64, d2);    // dx = +1 block: consumed by the lane below (m - 1)
-    if (kReadRes) sm100::tmem_ld16(tres, rr);
-    sm100::tmem_ld_wait();
-    // the accumulators are in registers: hand the TMEM slot back to the UMMA issuer
-    sm100::tc_fence_before();
-    __syncwarp();
-    if (c.lane == 0) sm100::mbar_arrive(&c.mb_tempty[slot]);
-    if (c.lane == 31) {
-      float4* q = reinterpret_cast<float4*>(xch + (wq * 2 + 0) * 16);
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-        q[i] = make_float4(__uint_as_float(a[4 * i]), __uint_as_float(a[4 * i + 1]), __uint_as_float(a[4 * i + 2]),
-                           __uint_as_float(a[4 * i + 3]));
-    }
-    if (c.lane == 0) {
-      float4* q = reinterpret_cast<float4*>(xch + (wq * 2 + 1) * 16);
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-        q[i] = make_float4(__uint_as_float(d2[4 * i]), __uint_as_float(d2[4 * i + 1]), __uint_as_float(d2[4 * i + 2]),
-                           __uint_as_float(d2[4 * i + 3]));
-    }
-    quad_sync(half);
-    // out[v] = D[v-1][dx=-1] + D[v][dx=0] + D[v+1][dx=+1]
-    float up[16], dn[16];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      up[i] = __shfl_up_sync(0xffffffffu, __uint_as_float(a[i]), 1);      // from lane - 1
-      dn[i] = __shfl_down_sync(0xffffffffu, __uint_as_float(d2[i]), 1);   // from lane + 1
-    }
-    if (c.lane == 0 && wq > 0) {     // row m - 1 lives in the previous warp
-      const float4* q = reinterpret_cast<const float4*>(xch + ((wq - 1) * 2 + 0) * 16);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float4 t = q[i];
-        up[4 * i] = t.x; up[4 * i + 1] = t.y; up[4 * i + 2] = t.z; up[4 * i + 3] = t.w;
-      }
-    }
-    if (c.lane == 31 && wq < 3) {    // row m + 1 lives in the next warp
-      const float4* q = reinterpret_cast<const float4*>(xch + ((wq + 1) * 2 + 1) * 16);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float4 t = q[i];
-        dn[4 * i] = t.x; dn[4 * i + 1] = t.y; dn[4 * i + 2] = t.z; dn[4 * i + 3] = t.w;
-      }
-    }
     // SAME padding in x: at x = 0 / x = fx-1 row v-1 / v+1 belongs to the neighbouring line (mask 0);
     // all partial sums are finite (pad rows multiply zero activations), so 0 * value is exact
     const float m_up = x == 0 ? 0.f : 1.f, m_dn = x == g.fx - 1 ? 0.f : 1.f;
-    float v[16];
+    float* res = ch.res + ((size_t)tile * kTileM + m) * kFeat + 8 * t;
+    float rr[8];
+    if (kReadRes) {
+      const float4 r0 = __ldcg(reinterpret_cast<const float4*>(res)), r1 = __ldcg(reinterpret_cast<const float4*>(res) + 1);
+      rr[0] = r0.x; rr[1] = r0.y; rr[2] = r0.z; rr[3] = r0.w; rr[4] = r1.x; rr[5] = r1.y; rr[6] = r1.z; rr[7] = r1.w;
+    }
+    float v[8];
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const float4 bi = bias4[i];
-      const float bias[4] = {bi.x, bi.y, bi.z, bi.w};
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int q = 4 * i + e;
-        const float acc = fmaf(up[q], m_up, fmaf(dn[q], m_dn, __uint_as_float(b[q])));
-        v[q] = X2 ? fmaf(acc, kUnscale, bias[e]) : acc + bias[e];
-        if (kReadRes) v[q] += __uint_as_float(rr[q]);
-      }
+    for (int q = 0; q < 8; ++q) {
+      const float acc = fmaf(up[h][q], m_up, fmaf(dn[h][q], m_dn, ACC(1, h, q)));
+      const float b = bias[8 * (q >> 1) + (q & 1)];
+      v[q] = X2 ? fmaf(acc, kUnscale, b) : acc + b;
+      if (kReadRes) v[q] += rr[q];
     }
     if (kWriteRes) {
       // rows outside the FoV carry values nobody reads; storing them unconditionally keeps the warp converged
-#pragma unroll
-      for (int q = 0; q < 16; ++q) rr[q] = __float_as_uint(v[q]);
-      sm100::tmem_st16(tres, rr);
+      __stcg(reinterpret_cast<float4*>(res), make_float4(v[0], v[1], v[2], v[3]));
+      __stcg(reinterpret_cast<float4*>(res) + 1, make_float4(v[4], v[5], v[6], v[7]));
     }
     if (KIND != EPI_LAST) {
       if (valid) {
-        // out = relu(.) as fp16: the ReLU rides on the conversion (cvt.rn.relu.f16x2.f32)
-        __half* dst = out_base + (size_t)r * 8;   // [k-chunk][row][8 halfs]; this half owns chunks 2*half, 2*half+1
+        // out = relu(.) as fp16: the ReLU rides on the conversion (cvt.rn.relu.f16x2.f32); channels 8 i + 2 t, +1 are
+        // one half2 of k-chunk i ([k-chunk][row][8 halfs])
+        __half* dst = ch.act_h[layer & 1] + ((size_t)g.guard + r) * 8 + 2 * t;
 #pragma unroll
-        for (int q = 0; q < 2; ++q) {
-          uint4 o;
-          o.x = sm100::cvt_relu_f16x2(v[8 * q + 0], v[8 * q + 1]);
-          o.y = sm100::cvt_relu_f16x2(v[8 * q + 2], v[8 * q + 3]);
-          o.z = sm100::cvt_relu_f16x2(v[8 * q + 4], v[8 * q + 5]);
-          o.w = sm100::cvt_relu_f16x2(v[8 * q + 6], v[8 * q + 7]);
-          *reinterpret_cast<uint4*>(dst + q * chunk_stride) = o;
+        for (int i = 0; i < 4; ++i) {
+          const uint32_t o = sm90::cvt_relu_f16x2(v[2 * i], v[2 * i + 1]);
+          *reinterpret_cast<uint32_t*>(dst + i * chunk_stride) = o;
           if (X2) {   // lo parts of relu(v): relu(v) - fp16(relu(v)) is exact in fp32
-            const uint32_t hi[4] = {o.x, o.y, o.z, o.w};
-            uint32_t lo[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hi[e]));
-              const __half2 l = __floats2half2_rn(fmaxf(v[8 * q + 2 * e], 0.f) - hf.x, fmaxf(v[8 * q + 2 * e + 1], 0.f) - hf.y);
-              lo[e] = *reinterpret_cast<const uint32_t*>(&l);
-            }
-            *reinterpret_cast<uint4*>(out_lo_base + (size_t)r * 8 + q * chunk_stride) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+            const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&o));
+            const __half2 l = __floats2half2_rn(fmaxf(v[2 * i], 0.f) - hf.x, fmaxf(v[2 * i + 1], 0.f) - hf.y);
+            *reinterpret_cast<__half2*>(p.ws.act_l[layer & 1] + ((size_t)g.guard + r) * 8 + 2 * t + i * chunk_stride) = l;
           }
         }
       }
     } else {
-      // conv_lom: this half's share of <relu(net), w_lom>; combine the halves, then logits = seed + update
-      const float* wl = c.s_bias + g.nconv * 32;
+      // conv_lom: this thread's share of <relu(net), w_lom>, summed over the four lanes that hold the row
+      const float* wl = c.s_bias + g.nconv * 32 + 2 * t;
       float part = 0.f;
 #pragma unroll
-      for (int q = 0; q < 16; ++q) part = fmaf(fmaxf(v[q], 0.f), wl[half * 16 + q], part);
-      float* dot = c.s_dot + (c.epi_cnt & 1) * kTileM;
-      if (half == 1) dot[m] = part;
-      asm volatile("bar.sync 3, 256;" ::: "memory");
-      if (half == 0 && valid) {
-        const float upd = part + dot[m] + wl[32];
+      for (int q = 0; q < 8; ++q) part = fmaf(fmaxf(v[q], 0.f), wl[8 * (q >> 1) + (q & 1)], part);
+      part += __shfl_xor_sync(0xffffffffu, part, 1);
+      part += __shfl_xor_sync(0xffffffffu, part, 2);
+      if (t == 0 && valid) {
+        const float upd = part + c.s_bias[g.nconv * 32 + 32];
         const float raw = raw_in[r];
         const float fed = isnan(raw) ? p.cv.opt.pad_value : raw;
         const float logit = fed + upd;
@@ -562,12 +551,18 @@ __device__ __forceinline__ int tc_epilogue(Ctx& c, int k, int layer, int ntiles)
         hit += step_counts(p, raw, logit);
       }
     }
-    if (kWriteRes) sm100::tmem_st_wait();
-    if (c.tid == 0) prof_add(c, 5, prof_now(c) - t0);
-    if (c.tid == 0) trace_ev(c, 6, c.epi_cnt);
-    ++c.epi_cnt;
   }
+#undef ACC
+  ++c.epi_cnt;
   return hit;
+}
+
+template <bool X2>
+__device__ __forceinline__ int tc_epilogue_any(Ctx& c, int k, int layer, int j, const float (&d)[kAccRegs]) {
+  if (layer == c.p->g.nconv - 1) return tc_epilogue<EPI_LAST, X2>(c, k, layer, j, d);
+  if (!(layer & 1)) return tc_epilogue<EPI_A, X2>(c, k, layer, j, d);
+  if (layer == 1) return tc_epilogue<EPI_B_FIRST, X2>(c, k, layer, j, d);
+  return tc_epilogue<EPI_B, X2>(c, k, layer, j, d);
 }
 
 // Adds the per-row counts of the last layer (this warp's `hit`) to the chain's step counters.
@@ -575,7 +570,7 @@ __device__ __forceinline__ void publish_counts(Ctx& c, int k, int hit) {
   hit = __reduce_add_sync(0xffffffffu, hit);
   if (c.lane == 0 && hit) atomicAdd(&c.s_misc[k], hit);
   asm volatile("bar.sync 5, 256;" ::: "memory");
-  if (c.tid == 0 && c.s_misc[k]) {   // packed per-CTA sums (step_counts): <= 882 rows per CTA, so no carry
+  if (c.tid == 0 && c.s_misc[k]) {   // packed per-CTA sums (step_counts): < 2^16 rows per CTA (kMaxTilesPerCta), so no carry
     const unsigned packed = (unsigned)c.s_misc[k];
     unsigned* cnt = c.p->ch[k].count + 2 * (c.round & 1u);
     if (packed & 0xffffu) atomicAdd(cnt, packed & 0xffffu);
@@ -585,15 +580,16 @@ __device__ __forceinline__ void publish_counts(Ctx& c, int k, int hit) {
 
 // One round of the conv stacks of the chains in `mask`, as ONE warp-specialised pipeline over the work
 // items (layer, chain, tile) in that order:
-//   warp 8  TMA producer : waits for the chain's split-phase barrier (previous layer complete in every
-//                          CTA), then per tile twelve 1-D bulk copies (3 z-planes x 4 k-chunks of 126 + 2*halo
-//                          rows; or ONE tiled TMA through the buffer's tensor map, FFN_B200_TMAP=1) into a
-//                          kActStages-stage shared-memory ring            full[stage]  <-  empty[stage]
-//   warp 9  UMMA issuer  : 18 UMMAs 128x96x16 per tile into a kAccSlots-slot TMEM ring; one commit frees the
-//                          smem stage, one publishes the slot           tfull[slot]  <-  tempty[slot]
-//   warps 0-7 epilogue   : every tile by all eight warps (2 channel halves x 4 TMEM lane quarters); after a
-//                          chain's tiles of a layer they ARRIVE at that chain's barrier and go on
-// A layer's weights are shared by all chains (double-buffered, the next layer prefetched once every UMMA of
+//   warp 8    TMA producer : waits for the chain's split-phase barrier (previous layer complete in every
+//                            CTA), then per tile twelve 1-D bulk copies (3 z-planes x 4 k-chunks of 126 + 2*halo
+//                            rows; or ONE tiled TMA through the buffer's tensor map, FFN_B200_TMAP=1) into a
+//                            kActStages-stage shared-memory ring            full[stage]  <-  empty[stage]
+//   warps 0-7 consumers    : two warpgroups, 64 accumulator rows of every tile each: 18 MMAs 64x96x16 (wgmma), then
+//                            the stage is released (one arrival per warp) and the epilogue runs from the
+//                            registers; after a chain's tiles of a layer every warp ARRIVES at that chain's
+//                            barrier and goes on
+//   warp 9    signaller    : turns the eight arrivals into the chain's gpu-scope release
+// A layer's weights are shared by all chains (double-buffered, the next layer prefetched once every MMA of
 // the layer before has completed).
 __device__ __forceinline__ void layers_pipelined(Ctx& c, unsigned mask) {
   const KParams& p = *c.p;
@@ -605,20 +601,19 @@ __device__ __forceinline__ void layers_pipelined(Ctx& c, unsigned mask) {
   const int nconv = g.nconv;
   const long long t_layers = prof_now(c);
 
-  // The two single-issuer roles run with the WHOLE warp converged (c.warp is warp-uniform by
-  // construction, see the kernel entry) and elect one lane only for the instructions with side effects:
-  // addresses and descriptors then live in uniform registers, instead of being broadcast from one
-  // lane's registers (ELECT / R2UR loop) in front of every bulk copy and every UMMA.
+  // The producer runs with the WHOLE warp converged (c.warp is warp-uniform by construction, see the kernel
+  // entry) and elects one lane only for the instructions with side effects: addresses then live in uniform
+  // registers, instead of being broadcast from one lane's registers in front of every bulk copy.
   if (c.warp == kLoadWarp) {
     // ------------------------------------------------------------------ TMA producer
     for (int layer = 0; layer < nconv; ++layer) {
       const int nch = layer == 0 ? 2 : 4;
       // The next layer's weights (next round's layer 0 after the last layer) are prefetched into the other
-      // buffer during this layer.  That buffer's previous user — layer - 1 — must have completed every UMMA,
-      // i.e. the tile issued just before this layer's first one (n0 - 1; commits are in order), and that is
-      // exactly what the `empty` wait of this layer's kActStages-th tile waits for (same stage).  A layer with
-      // fewer tiles waits for that phase explicitly at its end (it cannot have been overtaken: the stage's next
-      // user has not been loaded).
+      // buffer during this layer.  That buffer's previous user — layer - 1 — must have completed every MMA,
+      // i.e. the tile consumed just before this layer's first one (n0 - 1; every consumer warp works through the
+      // tiles in order), and that is exactly what the `empty` wait of this layer's kActStages-th tile waits for
+      // (same stage).  A layer with fewer tiles waits for that phase explicitly at its end (it cannot have been
+      // overtaken: the stage's next user has not been loaded).
       const unsigned n0 = c.load_cnt;   // first tile of this layer
       bool weights_pending = true;
       for (int k = 0; k < kMaxChains; ++k) {
@@ -628,30 +623,30 @@ __device__ __forceinline__ void layers_pipelined(Ctx& c, unsigned mask) {
         chain_wait(c, k, (unsigned)layer + 1u);   // event 1 = staged, event l + 1 = layer l - 1 complete everywhere
         if (c.lane == 0) trace_ev(c, 0, c.load_cnt);
 #ifndef FFN_EXP_NO_READER_FENCE
-        sm100::fence_proxy_async_global();
+        sm90::fence_proxy_async_global();
 #endif        // other CTAs' generic-proxy stores (ordered by the acquire) -> async proxy
         for (int j = 0; j < ntiles; ++j) {
           const int s = c.load_cnt % kActStages;
           mbar_wait(c, &c.mb_empty[s], ((c.load_cnt / kActStages) & 1u) ^ 1u);
           if (weights_pending && c.load_cnt - n0 == (unsigned)(kActStages - 1)) {
             weights_pending = false;
-            if (sm100::elect_one()) tc_issue_weight_load(c, (layer + 1 == nconv) ? 0 : layer + 1);
+            if (sm90::elect_one()) tc_issue_weight_load(c, (layer + 1 == nconv) ? 0 : layer + 1);
             __syncwarp();
           }
           const int r0 = (c.t_begin + j) * kTileOut;
           unsigned char* dst = act_smem + (size_t)s * stage_bytes;
-          if (sm100::elect_one()) {
-            sm100::mbar_expect_tx(&c.mb_full[s], (uint32_t)(3 * nch * seg_rows * 16));
+          if (sm90::elect_one()) {
+            sm90::mbar_expect_tx(&c.mb_full[s], (uint32_t)(3 * nch * seg_rows * 16));
             if (p.use_tmap) {
               // one tiled TMA: box (8 halfs, seg_rows rows, 3 z-planes, nch k-chunks) -> stage layout [k-chunk][dz][row]
-              sm100::tma_load_4d(dst, &p.tmap[k][layer == 0 ? 0 : 1 + ((layer - 1) & 1)], 0, g.guard + r0 - g.halo - g.pp, 0, 0,
-                                 &c.mb_full[s]);
+              sm90::tma_load_4d(dst, &p.tmap[k][layer == 0 ? 0 : 1 + ((layer - 1) & 1)], 0, g.guard + r0 - g.halo - g.pp, 0, 0,
+                                &c.mb_full[s]);
             } else {
               for (int cc = 0; cc < nch; ++cc)
                 for (int dzi = 0; dzi < 3; ++dzi)
-                  sm100::bulk_g2s(dst + (size_t)(cc * 3 + dzi) * seg_rows * 16,
-                                  in + ((size_t)cc * g.rows_alloc + g.guard + r0 + (dzi - 1) * g.pp - g.halo) * 8,
-                                  (uint32_t)seg_rows * 16, &c.mb_full[s]);
+                  sm90::bulk_g2s(dst + (size_t)(cc * 3 + dzi) * seg_rows * 16,
+                                 in + ((size_t)cc * g.rows_alloc + g.guard + r0 + (dzi - 1) * g.pp - g.halo) * 8,
+                                 (uint32_t)seg_rows * 16, &c.mb_full[s]);
             }
           }
           __syncwarp();
@@ -661,52 +656,8 @@ __device__ __forceinline__ void layers_pipelined(Ctx& c, unsigned mask) {
       }
       if (weights_pending) {
         if (n0 > 0) mbar_wait(c, &c.mb_empty[(n0 - 1u) % kActStages], ((n0 - 1u) / kActStages) & 1u);
-        if (sm100::elect_one()) tc_issue_weight_load(c, (layer + 1 == nconv) ? 0 : layer + 1);
+        if (sm90::elect_one()) tc_issue_weight_load(c, (layer + 1 == nconv) ? 0 : layer + 1);
         __syncwarp();
-      }
-    }
-  } else if (c.warp == kMmaWarp) {
-    // ------------------------------------------------------------------ UMMA issuer
-    for (int layer = 0; layer < nconv; ++layer) {
-      const int buf = layer & 1;
-      long long t0 = prof_now(c);
-      mbar_wait(c, &c.mb_w[buf], (c.bits >> buf) & 1u);
-      c.bits ^= 1u << buf;
-      if (c.lane == 0) prof_add(c, 2, prof_now(c) - t0);
-      const uint32_t b_lo = ((sm100::smem_u32(c.smem + buf * (27 * 4 * 512)) >> 4) & 0x3FFFu) | ((12u * 128u >> 4) << 16);
-      for (int k = 0; k < kMaxChains; ++k) {
-        if (!((mask >> k) & 1u)) continue;
-        for (int j = 0; j < ntiles; ++j) {
-          const int s = c.mma_cnt % kActStages, slot = c.mma_cnt % kAccSlots;
-#ifdef FFN_EXP_TEMPTY_FIRST
-          mbar_wait(c, &c.mb_tempty[slot], ((c.mma_cnt / kAccSlots) & 1u) ^ 1u);
-#endif
-          t0 = prof_now(c);
-          mbar_wait(c, &c.mb_full[s], (c.mma_cnt / kActStages) & 1u);
-          if (c.lane == 0) prof_add(c, 1, prof_now(c) - t0);
-          if (c.lane == 0) trace_ev(c, 2, c.mma_cnt);
-#ifndef FFN_EXP_TEMPTY_FIRST
-          mbar_wait(c, &c.mb_tempty[slot], ((c.mma_cnt / kAccSlots) & 1u) ^ 1u);
-#endif
-          sm100::tc_fence_after();
-          if (c.lane == 0) trace_ev(c, 3, c.mma_cnt);
-          t0 = prof_now(c);
-          const uint32_t a_lo = ((sm100::smem_u32(act_smem + (size_t)s * stage_bytes) >> 4) & 0x3FFFu) | ((uint32_t)(3 * seg_rows) << 16);
-          const uint32_t d = c.tmem_base + (uint32_t)(slot * kStackN);
-          if (sm100::elect_one()) {
-            if (layer == 0) {
-              tc_issue_tile<2>(d, a_lo, b_lo, seg_rows, g.xp);
-            } else {
-              tc_issue_tile<4>(d, a_lo, b_lo, seg_rows, g.xp);
-            }
-            sm100::umma_commit(&c.mb_tfull[slot]);   // accumulators of this tile complete
-            sm100::umma_commit(&c.mb_empty[s]);      // ... and its shared-memory stage is free again
-          }
-          __syncwarp();
-          if (c.lane == 0) prof_add(c, 3, prof_now(c) - t0);
-          if (c.lane == 0) trace_ev(c, 4, c.mma_cnt);
-          ++c.mma_cnt;
-        }
       }
     }
   } else if (c.warp == kSigWarp) {
@@ -722,29 +673,54 @@ __device__ __forceinline__ void layers_pipelined(Ctx& c, unsigned mask) {
 #endif
       }
   } else {
-    // ------------------------------------------------------------------ epilogue (warps 0-7)
+    // ------------------------------------------------------------------ consumers (warps 0-7)
+    const uint32_t wg_rows = (uint32_t)((c.warp >> 2) * 64);   // this warpgroup's first accumulator row (16-byte units)
     for (int layer = 0; layer < nconv; ++layer) {
-      const bool last = layer == nconv - 1;
+      const int buf = layer & 1;
+      long long t0 = prof_now(c);
+      mbar_wait(c, &c.mb_w[buf], bit_get(c, buf));
+      bit_flip(c, buf);
+      if (c.tid == 0) prof_add(c, 2, prof_now(c) - t0);
+      const uint32_t b_lo = ((sm90::smem_u32(c.smem + buf * (27 * 4 * 512)) >> 4) & 0x3FFFu) | ((12u * 128u >> 4) << 16);
       for (int k = 0; k < kMaxChains; ++k) {
         if (!((mask >> k) & 1u)) continue;
-        if (last) {
-          const int hit = tc_epilogue<EPI_LAST>(c, k, layer, ntiles);
+        int hit = 0;
+        for (int j = 0; j < ntiles; ++j) {
+          const int s = c.epi_cnt % kActStages;
+          t0 = prof_now(c);
+          mbar_wait(c, &c.mb_full[s], (c.epi_cnt / kActStages) & 1u);
+          if (c.tid == 0) prof_add(c, 1, prof_now(c) - t0);
+          if (c.tid == 0) trace_ev(c, 2, c.epi_cnt);
+          t0 = prof_now(c);
+          const uint32_t a_lo = (((sm90::smem_u32(act_smem + (size_t)s * stage_bytes) >> 4) & 0x3FFFu) + wg_rows) |
+                                ((uint32_t)(3 * seg_rows) << 16);
+          float d[kAccRegs];
+#pragma unroll
+          for (int i = 0; i < kAccRegs; ++i) d[i] = 0.f;
+          if (layer == 0) {
+            tc_mma_tile<2>(d, a_lo, b_lo, seg_rows, g.xp);
+          } else {
+            tc_mma_tile<4>(d, a_lo, b_lo, seg_rows, g.xp);
+          }
+          __syncwarp();
+          if (c.lane == 0) sm90::mbar_arrive(&c.mb_empty[s]);   // this warp's MMAs have read the stage
+          if (c.tid == 0) prof_add(c, 3, prof_now(c) - t0);
+          if (c.tid == 0) trace_ev(c, 4, c.epi_cnt);
+          t0 = prof_now(c);
+          hit += tc_epilogue_any<false>(c, k, layer, j, d);
+          if (c.tid == 0) prof_add(c, 5, prof_now(c) - t0);
+          if (c.tid == 0) trace_ev(c, 6, c.epi_cnt - 1u);
+        }
+        if (layer == nconv - 1) {
           publish_counts(c, k, hit);          // the round ends with a grid barrier: no chain arrival needed
         } else {
-          if (!(layer & 1)) {
-            tc_epilogue<EPI_A>(c, k, layer, ntiles);
-          } else if (layer == 1) {
-            tc_epilogue<EPI_B_FIRST>(c, k, layer, ntiles);
-          } else {
-            tc_epilogue<EPI_B>(c, k, layer, ntiles);
-          }
           chain_arrive_epi(c, k);
         }
       }
     }
   }
   // role-independent bookkeeping, identical in every thread (the weight-barrier parities, bits 0 / 1, are
-  // tracked by the UMMA issuer warp alone: nobody else waits on those barriers)
+  // tracked by the consumer warps alone: nobody else waits on those barriers)
   bit_set(c, 8, true);   // the last layer prefetched layer 0's weights of the next round into buffer 0
 #pragma unroll
   for (int k = 0; k < kMaxChains; ++k)
@@ -753,7 +729,7 @@ __device__ __forceinline__ void layers_pipelined(Ctx& c, unsigned mask) {
 }
 
 // Near-fp32 tensor-core layer (FFN_COMPUTE_FP16X2_TC): activations and weights are both split into fp16
-// hi + lo parts and every (tap-row, k-pair) becomes THREE UMMAs into the same fp32 accumulator,
+// hi + lo parts and every (tap-row, k-pair) becomes THREE MMAs into the same fp32 accumulator,
 //   a * w  ~=  a_hi * w_hi + a_lo * w_hi + a_hi * w_lo        (the dropped a_lo * w_lo term is ~2^-22 relative),
 // which gives ~22 significant bits per product.  One chain (chain 0), whole-grid barriers between layers;
 // shared memory is used differently from the fp16 path: activation stage 0 holds the hi parts and stage 1
@@ -774,85 +750,51 @@ __device__ __forceinline__ void tc_layer_x2(Ctx& c, int layer) {
   int hit = 0;
   bit_set(c, 8, true);
   if (c.warp == kLoadWarp) {
-    sm100::fence_proxy_async_global();
-    if (sm100::elect_one()) {
-      // both halves of this layer's weights; every UMMA of the previous layer has completed (its
-      // epilogue waited for the accumulators), so the buffers are free
+    sm90::fence_proxy_async_global();
+    if (sm90::elect_one()) {
+      // both halves of this layer's weights; every MMA of the previous layer has completed (its
+      // epilogue ran after them), so the buffers are free
       const uint32_t wbytes = (uint32_t)(27 * nch * 512);
       const __half* src = p.w.w16x2 + 2 * w16_layer_offset_halfs(layer);
-      sm100::mbar_expect_tx(&c.mb_w[0], 2 * wbytes);
-      sm100::bulk_g2s(c.smem, src, wbytes, &c.mb_w[0]);
-      sm100::bulk_g2s(c.smem + 27 * 4 * 512, src + wbytes / 2, wbytes, &c.mb_w[0]);
+      sm90::mbar_expect_tx(&c.mb_w[0], 2 * wbytes);
+      sm90::bulk_g2s(c.smem, src, wbytes, &c.mb_w[0]);
+      sm90::bulk_g2s(c.smem + 27 * 4 * 512, src + wbytes / 2, wbytes, &c.mb_w[0]);
     }
     __syncwarp();
     for (int j = 0; j < ntiles; ++j) {
       if (j > 0) mbar_wait(c, &c.mb_empty[0], (c.load_cnt & 1u) ^ 1u);
       const int r0 = (c.t_begin + j) * kTileOut;
-      if (sm100::elect_one()) {
-        sm100::mbar_expect_tx(&c.mb_full[0], (uint32_t)(2 * 3 * nch * seg_rows * 16));
+      if (sm90::elect_one()) {
+        sm90::mbar_expect_tx(&c.mb_full[0], (uint32_t)(2 * 3 * nch * seg_rows * 16));
         for (int part = 0; part < 2; ++part) {
           const __half* in = part ? in_lo : in_hi;
           unsigned char* dst = act_smem + (size_t)part * stage_bytes;
           for (int dzi = 0; dzi < 3; ++dzi)
             for (int cc = 0; cc < nch; ++cc)
-              sm100::bulk_g2s(dst + (size_t)(dzi * nch + cc) * seg_rows * 16,
-                              in + ((size_t)cc * g.rows_alloc + g.guard + r0 + (dzi - 1) * g.pp - g.halo) * 8,
-                              (uint32_t)seg_rows * 16, &c.mb_full[0]);
+              sm90::bulk_g2s(dst + (size_t)(dzi * nch + cc) * seg_rows * 16,
+                             in + ((size_t)cc * g.rows_alloc + g.guard + r0 + (dzi - 1) * g.pp - g.halo) * 8,
+                             (uint32_t)seg_rows * 16, &c.mb_full[0]);
         }
       }
       __syncwarp();
       ++c.load_cnt;
     }
-  } else if (c.warp == kMmaWarp) {
-    mbar_wait(c, &c.mb_w[0], bit_get(c, 0));
-    const uint32_t idesc = sm100::umma_idesc_f16(kTileM, kStackN);
-    const uint64_t hi = (uint64_t)((128u >> 4) | (1u << 14)) << 32;
-    const uint32_t bw_hi = ((sm100::smem_u32(c.smem) >> 4) & 0x3FFFu) | ((12u * 128u >> 4) << 16);
-    const uint32_t bw_lo = ((sm100::smem_u32(c.smem + 27 * 4 * 512) >> 4) & 0x3FFFu) | ((12u * 128u >> 4) << 16);
-    const uint32_t aa_hi = ((sm100::smem_u32(act_smem) >> 4) & 0x3FFFu) | ((uint32_t)seg_rows << 16);
-    const uint32_t aa_lo = ((sm100::smem_u32(act_smem + stage_bytes) >> 4) & 0x3FFFu) | ((uint32_t)seg_rows << 16);
-    for (int j = 0; j < ntiles; ++j) {
-      const int slot = c.mma_cnt % kAccSlots;
-      mbar_wait(c, &c.mb_full[0], c.mma_cnt & 1u);
-      mbar_wait(c, &c.mb_tempty[slot], ((c.mma_cnt / kAccSlots) & 1u) ^ 1u);
-      sm100::tc_fence_after();
-      const uint32_t d = c.tmem_base + (uint32_t)(slot * kStackN);
-      if (sm100::elect_one()) {
-        // The tensor core truncates when it aligns an MMA's sum to the accumulator, so the error of every
-        // accumulation scales with the accumulator's magnitude: the small cross terms (a_lo*w_hi, a_hi*w_lo,
-        // ~2^-11 of the result) go in FIRST, while the accumulator is small, the 9*nch/2 main MMAs last.
-#pragma unroll 1
-        for (int pass = 0; pass < 2; ++pass) {
-#pragma unroll 1
-          for (int row = 0; row < 9; ++row) {
-            const int tz = row / 3, ty = row % 3;
-            for (int jj = 0; jj < nch / 2; ++jj) {
-              const uint32_t aoff = (uint32_t)((tz * nch + 2 * jj) * seg_rows + ty * g.xp);
-              const uint32_t boff = (uint32_t)((row * nch + 2 * jj) * (12 * 128 / 16));
-              if (pass == 0) {
-                sm100::umma_f16(d, hi | (uint64_t)(aa_lo + aoff), hi | (uint64_t)(bw_hi + boff), idesc, (row | jj) != 0 ? 1u : 0u);
-                sm100::umma_f16(d, hi | (uint64_t)(aa_hi + aoff), hi | (uint64_t)(bw_lo + boff), idesc, 1u);
-              } else {
-                sm100::umma_f16(d, hi | (uint64_t)(aa_hi + aoff), hi | (uint64_t)(bw_hi + boff), idesc, 1u);
-              }
-            }
-          }
-        }
-        sm100::umma_commit(&c.mb_tfull[slot]);
-        sm100::umma_commit(&c.mb_empty[0]);
-      }
-      __syncwarp();
-      ++c.mma_cnt;
-    }
   } else if (c.warp < 8) {
-    if (last) {
-      hit = tc_epilogue<EPI_LAST, true>(c, 0, layer, ntiles);
-    } else if (!(layer & 1)) {
-      tc_epilogue<EPI_A, true>(c, 0, layer, ntiles);
-    } else if (layer == 1) {
-      tc_epilogue<EPI_B_FIRST, true>(c, 0, layer, ntiles);
-    } else {
-      tc_epilogue<EPI_B, true>(c, 0, layer, ntiles);
+    mbar_wait(c, &c.mb_w[0], bit_get(c, 0));
+    const uint32_t wg_rows = (uint32_t)((c.warp >> 2) * 64);
+    const uint32_t bw_hi = ((sm90::smem_u32(c.smem) >> 4) & 0x3FFFu) | ((12u * 128u >> 4) << 16);
+    const uint32_t bw_lo = ((sm90::smem_u32(c.smem + 27 * 4 * 512) >> 4) & 0x3FFFu) | ((12u * 128u >> 4) << 16);
+    const uint32_t aa_hi = (((sm90::smem_u32(act_smem) >> 4) & 0x3FFFu) + wg_rows) | ((uint32_t)seg_rows << 16);
+    const uint32_t aa_lo = (((sm90::smem_u32(act_smem + stage_bytes) >> 4) & 0x3FFFu) + wg_rows) | ((uint32_t)seg_rows << 16);
+    for (int j = 0; j < ntiles; ++j) {
+      mbar_wait(c, &c.mb_full[0], c.epi_cnt & 1u);
+      float d[kAccRegs];
+#pragma unroll
+      for (int i = 0; i < kAccRegs; ++i) d[i] = 0.f;
+      tc_mma_tile_x2(d, aa_hi, aa_lo, bw_hi, bw_lo, nch, seg_rows, g.xp);
+      __syncwarp();
+      if (c.lane == 0) sm90::mbar_arrive(&c.mb_empty[0]);
+      hit += tc_epilogue_any<true>(c, 0, layer, j, d);
     }
     if (last) publish_counts(c, 0, hit);
   }
@@ -1734,7 +1676,7 @@ __device__ __forceinline__ int chain_advance(const Ctx& c, LChain L, Sched* sc, 
       if (c.lane == 0) {
         trace_event(p, st, EV_SEED_START, st->start[0], st->start[1], st->start[2]);
         st->ctr.segment_at_calls++;
-        st->seg_t0 = sm100::globaltimer_ns();
+        st->seg_t0 = sm90::globaltimer_ns();
         st->phase = PH_AFTER_CLEAR;
         st->popped = 0;
       }
@@ -1966,7 +1908,7 @@ __device__ __forceinline__ int chain_advance(const Ctx& c, LChain L, Sched* sc, 
             o.start_zyx[1] = st->start[1];
             o.start_zyx[2] = st->start[2];
             o.iters = st->iters;
-            o.walltime_sec = (double)(sm100::globaltimer_ns() - st->seg_t0) * 1e-9;
+            o.walltime_sec = (double)(sm90::globaltimer_ns() - st->seg_t0) * 1e-9;
             if (p.job.debug & 16) o.walltime_sec = L.k * 1e5 + st->start_max_id;   // experiments
             p.job.origins[sc->n_origins] = o;
           } else {
@@ -2025,7 +1967,7 @@ __device__ __forceinline__ void leader_round(Ctx& c, unsigned stepped) {
   // Watchdog: one launch covers at most 2^15 FoV steps (a few seconds).  A launch that is still going after
   // 60 s (FFN_B200_WATCHDOG_S; sanitizer runs need more) has stalled; raise the abort flag so that every CTA leaves
   // at this round boundary and the host reports it.
-  if (c.tid == 0 && sm100::globaltimer_ns() - c.t_start > (unsigned long long)p.job.watchdog_ns) atomicExch(p.ws.abort_flag, 5);
+  if (c.tid == 0 && sm90::globaltimer_ns() - c.t_start > (unsigned long long)p.job.watchdog_ns) atomicExch(p.ws.abort_flag, 5);
   // Work on shared-memory copies: the serial code is full of read-after-write on these fields, and in
   // global memory every one of those is an L2 round trip.
   for (int i = c.tid; i < K * kStateWords; i += 256) {
@@ -2151,7 +2093,7 @@ __device__ __forceinline__ void leader_round(Ctx& c, unsigned stepped) {
   __syncthreads();
   // everything above (ordered by bar.sync) becomes visible before the round is announced
   if (c.tid == 0) {
-    sm100::red_release_add(p.round_flag, 1u);
+    sm90::red_release_add(p.round_flag, 1u);
     prof_add(c, 8, prof_now(c) - t_all);
   }
 }
@@ -2297,14 +2239,12 @@ __device__ __forceinline__ void run_layers(Ctx& c, unsigned mask) {
   const KParams& p = *c.p;
   if (p.compute_mode == FFN_COMPUTE_FP16_TC) {
     // the staged operands: every thread's stores, then one arrival per chain (event 1 of the round)
-    sm100::tc_fence_before();
     __syncthreads();
     if (c.tid == 0) {
 #pragma unroll
       for (int k = 0; k < kMaxChains; ++k)
-        if ((mask >> k) & 1u) sm100::red_release_add(p.ch[k].bar, 1u);
+        if ((mask >> k) & 1u) sm90::red_release_add(p.ch[k].bar, 1u);
     }
-    sm100::tc_fence_after();
     layers_pipelined(c, mask);
   } else {
     layers_blocking(c);
@@ -2326,27 +2266,24 @@ __global__ void __launch_bounds__(kThreads, 1) ffn_flood_kernel(const __grid_con
   c.bar_target = 0;
   c.ev0 = c.ev1 = c.ev2 = c.ev3 = c.ev4 = 0;
   c.round = 0;
-  c.t_start = sm100::globaltimer_ns();
+  c.t_start = sm90::globaltimer_ns();
   c.smem = smem_raw;
   const SmemLayout L = smem_layout(p.g);
   c.s_bias = reinterpret_cast<float*>(smem_raw + L.bias);
   c.mb_w = reinterpret_cast<uint64_t*>(smem_raw + L.bars);
   c.mb_full = c.mb_w + 2;
   c.mb_empty = c.mb_full + kActStages;
-  c.mb_tfull = c.mb_empty + kActStages;
-  c.mb_tempty = c.mb_tfull + kAccSlots;
-  c.mb_sig = c.mb_tempty + kAccSlots;
-  c.s_tmem = reinterpret_cast<uint32_t*>(c.mb_sig + kMaxChains);
-  c.load_cnt = c.mma_cnt = c.epi_cnt = 0;
+  c.mb_sig = c.mb_empty + kActStages;
+  c.load_cnt = c.epi_cnt = 0;
   c.s_misc = reinterpret_cast<int*>(smem_raw + L.bars + kOffMisc);
   c.s_round = reinterpret_cast<int*>(smem_raw + L.bars + kOffRound);   // 2 * kMaxChains * 8 ints
   c.s_xchg = reinterpret_cast<float*>(smem_raw + L.bars + kOffXchg);
-  c.s_dot = c.s_xchg + 2 * 2 * 4 * 2 * 16;
   // CTA 0's working copies of the chain states and the scheduler block live in the epilogue's exchange area: they are
   // only used inside leader_round, between the grid barrier and the round's first tile
   c.s_state = reinterpret_cast<CanvasState*>(smem_raw + L.bars + kOffXchg);
   c.s_sched = reinterpret_cast<Sched*>(smem_raw + L.bars + kOffXchg + kMaxChains * kStateSlot);
-  static_assert((2 + 2 * kActStages + 2 * kAccSlots + kMaxChains) * 8 + 8 <= kOffMisc, "mbarrier area");
+  static_assert((2 + 2 * kActStages + kMaxChains) * 8 <= kOffMisc, "mbarrier area");
+  static_assert(kMaxChains * kStateSlot + (int)sizeof(Sched) <= kXchgBytes, "leader working copies");
   c.prof = nullptr;
   if (FFN_PROFILE && p.ws.prof && (c.cta == 0 || c.cta == c.G - 1)) {
     c.prof = reinterpret_cast<long long*>(smem_raw + L.bars + kOffProf);
@@ -2358,7 +2295,6 @@ __global__ void __launch_bounds__(kThreads, 1) ffn_flood_kernel(const __grid_con
 #endif
   const long long t_kernel = prof_now(c);
   c.bits = 0;
-  c.tmem_base = 0;
   const bool tc = p.compute_mode != FFN_COMPUTE_FP32;
   const int K = p.nchains;
 
@@ -2368,31 +2304,22 @@ __global__ void __launch_bounds__(kThreads, 1) ffn_flood_kernel(const __grid_con
   if (c.tid < 2 * kMaxChains * 8) c.s_round[c.tid] = 0;
   if (tc) {
     if (c.tid == 0) {
-      sm100::mbar_init(&c.mb_w[0], 1);
-      sm100::mbar_init(&c.mb_w[1], 1);
+      sm90::mbar_init(&c.mb_w[0], 1);
+      sm90::mbar_init(&c.mb_w[1], 1);
       for (int i = 0; i < kActStages; ++i) {
-        sm100::mbar_init(&c.mb_full[i], 1);
-        sm100::mbar_init(&c.mb_empty[i], 1);
+        sm90::mbar_init(&c.mb_full[i], 1);
+        sm90::mbar_init(&c.mb_empty[i], 8);   // one arrival per consumer warp
       }
-      for (int i = 0; i < kAccSlots; ++i) {
-        sm100::mbar_init(&c.mb_tfull[i], 1);
-        sm100::mbar_init(&c.mb_tempty[i], 8);   // one arrival per epilogue warp
-      }
-      for (int i = 0; i < kMaxChains; ++i) sm100::mbar_init(&c.mb_sig[i], 8);
-      sm100::fence_mbar_init();
+      for (int i = 0; i < kMaxChains; ++i) sm90::mbar_init(&c.mb_sig[i], 8);
+      sm90::fence_mbar_init();
     }
-    __syncwarp();
-    if (c.warp == 0) sm100::tmem_alloc<kTmemCols>(c.s_tmem);
-    sm100::tc_fence_before();
     __syncthreads();
-    sm100::tc_fence_after();
-    c.tmem_base = __shfl_sync(0xffffffffu, *c.s_tmem, 0);
     if (p.compute_mode == FFN_COMPUTE_FP16_TC) {   // the split mode loads both weight halves per layer
       if (c.warp == kLoadWarp && c.lane == 0) {
         tc_issue_weight_load(c, 0);
         if (p.use_tmap)
           for (int k = 0; k < p.nchains; ++k)
-            for (int i = 0; i < 3; ++i) sm100::tma_prefetch_desc(&p.tmap[k][i]);
+            for (int i = 0; i < 3; ++i) sm90::tma_prefetch_desc(&p.tmap[k][i]);
       }
       bit_set(c, 8, true);
     }
@@ -2414,7 +2341,7 @@ __global__ void __launch_bounds__(kThreads, 1) ffn_flood_kernel(const __grid_con
       for (int k = 0; k < K; ++k)
         if ((mask >> k) & 1u) tail_paste(c, k, 0, c.round & 1u, 0, 0, 0, b0 + k, false);
       ++c.round;
-      if (c.tid == 0) c.s_misc[kMiscAbort] = sm100::ld_volatile_s32(p.ws.abort_flag);   // one reader: no divergent exit
+      if (c.tid == 0) c.s_misc[kMiscAbort] = sm90::ld_volatile_s32(p.ws.abort_flag);   // one reader: no divergent exit
       __syncthreads();
       if (c.s_misc[kMiscAbort] != 0) break;
     }
@@ -2448,17 +2375,17 @@ __global__ void __launch_bounds__(kThreads, 1) ffn_flood_kernel(const __grid_con
       // ---- the leader's decisions for this round
       if (c.tid == 0) {
         spin_until(c, p.round_flag, c.round + 1u, 4);
-        c.s_misc[kMiscAbort] = sm100::ld_volatile_s32(p.ws.abort_flag);   // one reader: the whole CTA must take the same branch
+        c.s_misc[kMiscAbort] = sm90::ld_volatile_s32(p.ws.abort_flag);   // one reader: the whole CTA must take the same branch
       }
       __syncthreads();
       const int abort_now = c.s_misc[kMiscAbort];
       if (c.tid < K) {
         int* cur = c.s_round + 8 * c.tid;
-        cur[0] = sm100::ld_volatile_s32(&p.ctl->action[c.tid]);
-        cur[1] = sm100::ld_volatile_s32(&p.ctl->pos[c.tid][0]);
-        cur[2] = sm100::ld_volatile_s32(&p.ctl->pos[c.tid][1]);
-        cur[3] = sm100::ld_volatile_s32(&p.ctl->pos[c.tid][2]);
-        cur[4] = sm100::ld_volatile_s32(&p.ctl->buf[c.tid]);
+        cur[0] = sm90::ld_volatile_s32(&p.ctl->action[c.tid]);
+        cur[1] = sm90::ld_volatile_s32(&p.ctl->pos[c.tid][0]);
+        cur[2] = sm90::ld_volatile_s32(&p.ctl->pos[c.tid][1]);
+        cur[3] = sm90::ld_volatile_s32(&p.ctl->pos[c.tid][2]);
+        cur[4] = sm90::ld_volatile_s32(&p.ctl->buf[c.tid]);
       }
       __syncthreads();
       if (abort_now != 0) break;
@@ -2498,13 +2425,8 @@ __global__ void __launch_bounds__(kThreads, 1) ffn_flood_kernel(const __grid_con
   __syncthreads();
   if (c.prof && c.tid < 16) p.ws.prof[(c.cta == 0 ? 0 : 16) + c.tid] += c.prof[c.tid];
   // Teardown: no bulk copy may be in flight into this CTA's shared memory at exit (the fp16 path always
-  // has the next round's layer-0 weights in flight; only the UMMA issuer warp knows that barrier's parity).
-  if (tc) {
-    if (c.warp == kMmaWarp && bit_get(c, 8)) mbar_wait(c, &c.mb_w[0], bit_get(c, 0));
-    sm100::tc_fence_before();
-    __syncthreads();
-    if (c.warp == 0) sm100::tmem_dealloc<kTmemCols>(c.tmem_base);
-  }
+  // has the next round's layer-0 weights in flight; only the consumer warps know that barrier's parity).
+  if (tc && c.warp == 0 && bit_get(c, 8)) mbar_wait(c, &c.mb_w[0], bit_get(c, 0));
 }
 
 }  // namespace FFN_KNS

@@ -1,7 +1,7 @@
-// selftest.cuh — known-answer tests and micro-benchmarks of the sm_100a building blocks.
-// Not part of the product path: they pin the UMMA descriptor conventions the conv kernel relies on
+// selftest.cuh — known-answer tests and micro-benchmarks of the sm_90a building blocks.
+// Not part of the product path: they pin the wgmma descriptor conventions the conv kernel relies on
 // (K-major, no-swizzle core matrices; shifted start addresses = convolution taps) and measure the
-// numbers DESIGN.md's cycle model uses (UMMA issue rate vs N, grid-barrier latency, bulk-copy time).
+// grid-barrier latency and the bulk-copy time.
 #pragma once
 
 #include <cuda_fp16.h>
@@ -12,7 +12,7 @@
 #include <string>
 #include <vector>
 
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace ffn {
 namespace selftest {
@@ -20,104 +20,42 @@ namespace selftest {
 // Bounded spin: a broken descriptor must not hang the GPU box.
 __device__ __forceinline__ void bounded_wait(uint64_t* bar, uint32_t parity) {
   const long long t0 = clock64();
-  while (!sm100::mbar_try_wait(bar, parity)) {
+  while (!sm90::mbar_try_wait(bar, parity)) {
     if (clock64() - t0 > (1ll << 31)) return;
   }
 }
 
-// ---- variant 0: D[128 x 32] = A[128 x K] * B[32 x K]^T with explicit descriptors --------------
-// A in smem: [k-chunk][row] 16-byte units (row pitch 16 B, chunk pitch a_lbo); start address may be
-// shifted by `a_shift_rows` rows (a convolution tap).  B: [k-chunk][n-group][8][8].
-__global__ void umma_kat_kernel(const __half* a_g, int a_rows_total, const __half* b_g, int kchunks,
-                                int a_shift_rows, uint32_t a_lbo, uint32_t a_sbo, uint32_t b_lbo, uint32_t b_sbo,
-                                float* d_out) {
+// ---- variant 0: D[128 x 96] = A[128 x K] * B[96 x K]^T with explicit descriptors ------------
+// Two warpgroups, 64 rows each, like the conv kernel's consumers.  A in smem: [k-chunk][row] 16-byte
+// units (row pitch 16 B, chunk pitch a_lbo); start address shifted by `a_shift_rows` rows (a
+// convolution tap).  B: [k-chunk][12 n-groups][8][8].
+__global__ void wgmma_kat_kernel(const __half* a_g, int a_rows_total, const __half* b_g, int kchunks,
+                                 int a_shift_rows, uint32_t a_lbo, uint32_t a_sbo, uint32_t b_lbo, uint32_t b_sbo,
+                                 float* d_out) {
   extern __shared__ __align__(1024) unsigned char smem[];
   __half* a_s = reinterpret_cast<__half*>(smem);
   __half* b_s = a_s + (size_t)kchunks * a_rows_total * 8;
-  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + 196608);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + 196608 + 16);
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   for (int i = tid; i < kchunks * a_rows_total * 8; i += blockDim.x) a_s[i] = a_g[i];
-  for (int i = tid; i < kchunks * 32 * 8; i += blockDim.x) b_s[i] = b_g[i];
-  if (tid == 0) {
-    sm100::mbar_init(bar, 1);
-    sm100::fence_mbar_init();
-  }
-  __syncwarp();
-  if (warp == 0) sm100::tmem_alloc<32>(tmem_slot);
-  sm100::fence_proxy_async();   // generic-proxy smem writes -> visible to the tensor core (async proxy)
-  sm100::tc_fence_before();
+  for (int i = tid; i < kchunks * 96 * 8; i += blockDim.x) b_s[i] = b_g[i];
+  sm90::fence_proxy_async();   // generic-proxy smem writes -> visible to the tensor core (async proxy)
   __syncthreads();
-  sm100::tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  if (tid == 0) {
-    const uint32_t idesc = sm100::umma_idesc_f16(128, 32);
-    for (int j = 0; j < kchunks / 2; ++j) {
-      const uint32_t a_addr = sm100::smem_u32(a_s) + (uint32_t)((2 * j) * a_rows_total + a_shift_rows) * 16;
-      const uint32_t b_addr = sm100::smem_u32(b_s) + (uint32_t)(2 * j) * 512;
-      sm100::umma_f16(tmem, sm100::umma_desc(a_addr, a_lbo, a_sbo), sm100::umma_desc(b_addr, b_lbo, b_sbo), idesc,
-                      j > 0 ? 1u : 0u);
-    }
-    sm100::umma_commit(bar);
+  const int row0 = (warp >> 2) * 64;
+  float d[48];
+  for (int i = 0; i < 48; ++i) d[i] = 0.f;
+  sm90::wgmma_fence();
+  for (int j = 0; j < kchunks / 2; ++j) {
+    const uint32_t a_addr = sm90::smem_u32(a_s) + (uint32_t)((2 * j) * a_rows_total + a_shift_rows + row0) * 16;
+    const uint32_t b_addr = sm90::smem_u32(b_s) + (uint32_t)(2 * j) * 12 * 128;
+    sm90::wgmma_m64n96k16(d, sm90::wgmma_desc(a_addr, a_lbo, a_sbo), sm90::wgmma_desc(b_addr, b_lbo, b_sbo), j > 0 ? 1u : 0u);
   }
-  __syncwarp();
-  bounded_wait(bar, 0);
-  sm100::tc_fence_after();
-  if (warp < 4) {
-    uint32_t r[32];
-    sm100::tmem_ld32(tmem + ((uint32_t)(warp * 32) << 16), r);
-    sm100::tmem_ld_wait();
-    for (int k = 0; k < 32; ++k) d_out[(size_t)(warp * 32 + (tid & 31)) * 32 + k] = __uint_as_float(r[k]);
+  sm90::wgmma_commit();
+  sm90::wgmma_wait_all();
+  for (int i = 0; i < 48; ++i) {
+    const int row = row0 + (warp & 3) * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+    const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+    d_out[(size_t)row * 96 + col] = d[i];
   }
-  sm100::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) sm100::tmem_dealloc<32>(tmem);
-}
-
-// ---- variant 1: UMMA issue rate, A and B from shared memory ----------------------------------
-// M x N x 16 UMMAs issued back to back by one thread; NACC independent accumulators (rotating);
-// the A start address moves like a convolution tap.  Reports cycles per UMMA.
-template <int M, int N, int NACC>
-__global__ void umma_rate_kernel(int iters, long long* cycles_out) {
-  extern __shared__ __align__(1024) unsigned char smem[];
-  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + 98304);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + 98304 + 16);
-  const int tid = threadIdx.x, warp = tid >> 5;
-  for (int i = tid; i < 98304 / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(smem)[i] = 0x3c003c00u;  // 1.0h
-  if (tid == 0) {
-    sm100::mbar_init(bar, 1);
-    sm100::fence_mbar_init();
-  }
-  __syncwarp();
-  if (warp == 0) sm100::tmem_alloc<512>(tmem_slot);
-  sm100::fence_proxy_async();
-  sm100::tc_fence_before();
-  __syncthreads();
-  sm100::tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  if (tid == 0) {
-    const uint32_t idesc = sm100::umma_idesc_f16(M, N);
-    const uint32_t hi = (128u >> 4) | (1u << 14);
-    const uint32_t a_lo = ((sm100::smem_u32(smem) >> 4) & 0x3FFFu) | ((16384u >> 4) << 16);
-    const uint32_t b_lo = ((sm100::smem_u32(smem + 65536) >> 4) & 0x3FFFu) | (((uint32_t)N * 16u >> 4) << 16);
-    const uint64_t bd = ((uint64_t)hi << 32) | b_lo;
-    const long long t0 = clock64();
-    for (int i = 0; i < iters; i += 8) {
-#pragma unroll
-      for (int u = 0; u < 8; ++u) {
-        const uint64_t ad = ((uint64_t)hi << 32) | (uint64_t)(a_lo + (uint32_t)(((i + u) * 37) & 511));
-        sm100::umma_f16(tmem + (uint32_t)((u % NACC) * N), ad, bd, idesc, i > 0 ? 1u : 0u);
-      }
-    }
-    sm100::umma_commit(bar);
-    const long long t1 = clock64();
-    bounded_wait(bar, 0);
-    cycles_out[2 * blockIdx.x] = clock64() - t0;
-    cycles_out[2 * blockIdx.x + 1] = t1 - t0;   // issue-only time
-  }
-  sm100::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) sm100::tmem_dealloc<512>(tmem);
 }
 
 // ---- variant 2: grid-barrier latency --------------------------------------------------------
@@ -131,7 +69,7 @@ __global__ void barrier_kernel(unsigned* bar, int iters, long long* cycles_out) 
       __threadfence();
       atomicAdd(bar, 1u);
       const long long tw = clock64();
-      while (sm100::ld_acquire_u32(bar) < target) {
+      while (sm90::ld_acquire_u32(bar) < target) {
         if (clock64() - tw > (1ll << 31)) break;
       }
       __threadfence();
@@ -146,17 +84,17 @@ __global__ void bulk_kernel(const unsigned char* src, int pieces, int piece_byte
   extern __shared__ __align__(1024) unsigned char smem[];
   uint64_t* bar = reinterpret_cast<uint64_t*>(smem + 131072);
   if (threadIdx.x == 0) {
-    sm100::mbar_init(bar, 1);
-    sm100::fence_mbar_init();
+    sm90::mbar_init(bar, 1);
+    sm90::fence_mbar_init();
   }
   __syncthreads();
   uint32_t parity = 0;
   const long long t0 = clock64();
   for (int it = 0; it < iters; ++it) {
     if (threadIdx.x == 0) {
-      sm100::mbar_expect_tx(bar, (uint32_t)(pieces * piece_bytes));
+      sm90::mbar_expect_tx(bar, (uint32_t)(pieces * piece_bytes));
       for (int i = 0; i < pieces; ++i)
-        sm100::bulk_g2s(smem + (size_t)i * piece_bytes,
+        sm90::bulk_g2s(smem + (size_t)i * piece_bytes,
                         src + ((size_t)blockIdx.x * pieces + i) * piece_bytes + (size_t)(it & 7) * 16, (uint32_t)piece_bytes,
                         bar);
     }
@@ -165,54 +103,6 @@ __global__ void bulk_kernel(const unsigned char* src, int pieces, int piece_byte
     __syncthreads();
   }
   if (threadIdx.x == 0) cycles_out[blockIdx.x] = clock64() - t0;
-}
-
-// ---- variant 5: what does tcgen05.shift.down do? ------------------------------------------------
-// Lane l, column c of a 64-column TMEM block is filled with 1000 * c + l; after ONE
-// `tcgen05.shift.cta_group::1.down [base + col0]` every value is read back, so the host can tell which
-// lanes / columns moved (candidate for a shuffle-free epilogue: the dx taps of the stacked accumulator are
-// one row apart).  All waits bounded.
-__global__ void tmem_shift_probe_kernel(int col0, float* out) {
-  __shared__ uint64_t bar;
-  __shared__ uint32_t tmem_slot;
-  const int tid = threadIdx.x, warp = tid >> 5;
-  if (tid == 0) {
-    sm100::mbar_init(&bar, 1);
-    sm100::fence_mbar_init();
-  }
-  __syncwarp();
-  if (warp == 0) sm100::tmem_alloc<64>(&tmem_slot);
-  sm100::tc_fence_before();
-  __syncthreads();
-  sm100::tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  const uint32_t lane_base = tmem + ((uint32_t)(warp * 32) << 16);
-  for (int blk = 0; blk < 4; ++blk) {
-    uint32_t v[16];
-#pragma unroll
-    for (int k = 0; k < 16; ++k) v[k] = __float_as_uint(1000.f * (float)(blk * 16 + k) + (float)tid);
-    sm100::tmem_st16(lane_base + blk * 16, v);
-  }
-  sm100::tmem_st_wait();
-  sm100::tc_fence_before();
-  __syncthreads();
-  sm100::tc_fence_after();
-  if (tid == 0) {
-    asm volatile("tcgen05.shift.cta_group::1.down [%0];" ::"r"(tmem + (uint32_t)col0) : "memory");
-    sm100::umma_commit(&bar);
-  }
-  __syncwarp();
-  bounded_wait(&bar, 0);
-  sm100::tc_fence_after();
-  for (int blk = 0; blk < 4; ++blk) {
-    uint32_t v[16];
-    sm100::tmem_ld16(lane_base + blk * 16, v);
-    sm100::tmem_ld_wait();
-    for (int k = 0; k < 16; ++k) out[(size_t)tid * 64 + blk * 16 + k] = __uint_as_float(v[k]);
-  }
-  sm100::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) sm100::tmem_dealloc<64>(tmem);
 }
 
 inline float host_half_round(float v) { return __half2float(__float2half_rn(v)); }
@@ -228,7 +118,7 @@ inline float host_half_round(float v) { return __half2float(__float2half_rn(v));
 
 inline int run_kat(double* out, std::string* err) {
   const int K = 64, kch = K / 8, rows_total = 256;   // A window has room for shifts up to 127 rows
-  std::vector<float> a((size_t)rows_total * K), b((size_t)32 * K);
+  std::vector<float> a((size_t)rows_total * K), b((size_t)96 * K);
   unsigned s = 12345u;
   auto rnd = [&]() {
     s = s * 1664525u + 1013904223u;
@@ -236,39 +126,42 @@ inline int run_kat(double* out, std::string* err) {
   };
   for (auto& v : a) v = rnd();
   for (auto& v : b) v = rnd();
-  std::vector<__half> ah((size_t)kch * rows_total * 8), bh((size_t)kch * 32 * 8);
+  std::vector<__half> ah((size_t)kch * rows_total * 8), bh((size_t)kch * 96 * 8);
   for (int r = 0; r < rows_total; ++r)
     for (int k = 0; k < K; ++k) ah[((size_t)(k / 8) * rows_total + r) * 8 + k % 8] = __float2half_rn(a[(size_t)r * K + k]);
-  for (int n = 0; n < 32; ++n)
+  for (int n = 0; n < 96; ++n)
     for (int k = 0; k < K; ++k)
-      bh[(((size_t)(k / 8)) * 4 + n / 8) * 64 + (n % 8) * 8 + k % 8] = __float2half_rn(b[(size_t)n * K + k]);
+      bh[(((size_t)(k / 8)) * 12 + n / 8) * 64 + (n % 8) * 8 + k % 8] = __float2half_rn(b[(size_t)n * K + k]);
   __half *d_a = nullptr, *d_b = nullptr;
   float* d_d = nullptr;
   ST_CUDA(cudaMalloc(&d_a, ah.size() * 2));
   ST_CUDA(cudaMalloc(&d_b, bh.size() * 2));
-  ST_CUDA(cudaMalloc(&d_d, 128 * 32 * 4));
+  ST_CUDA(cudaMalloc(&d_d, 128 * 96 * 4));
   ST_CUDA(cudaMemcpy(d_a, ah.data(), ah.size() * 2, cudaMemcpyHostToDevice));
   ST_CUDA(cudaMemcpy(d_b, bh.data(), bh.size() * 2, cudaMemcpyHostToDevice));
-  ST_CUDA(cudaFuncSetAttribute(umma_kat_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 196608 + 64));
-  const uint32_t a_lbo = rows_total * 16, a_sbo = 128, b_lbo = 512, b_sbo = 128;
+  // the swapped-descriptor case strides 8-row groups by a_lbo / b_lbo and reaches ~58 KB past the operand base:
+  // allocate that much so the wrong answer is a wrong number, not an out-of-range shared-memory read
+  const int smem = 64 * 1024;
+  ST_CUDA(cudaFuncSetAttribute(wgmma_kat_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  const uint32_t a_lbo = rows_total * 16, a_sbo = 128, b_lbo = 12 * 128, b_sbo = 128;
   struct Case { int shift; bool swapped; };
   const Case cases[4] = {{0, false}, {3, false}, {35, false}, {0, true}};
   for (int ci = 0; ci < 4; ++ci) {
     const Case& c = cases[ci];
-    ST_CUDA(cudaMemset(d_d, 0xff, 128 * 32 * 4));
-    umma_kat_kernel<<<1, 128, 196608 + 64>>>(d_a, rows_total, d_b, kch, c.shift, c.swapped ? a_sbo : a_lbo,
+    ST_CUDA(cudaMemset(d_d, 0xff, 128 * 96 * 4));
+    wgmma_kat_kernel<<<1, 256, smem>>>(d_a, rows_total, d_b, kch, c.shift, c.swapped ? a_sbo : a_lbo,
                                        c.swapped ? a_lbo : a_sbo, c.swapped ? b_sbo : b_lbo,
                                        c.swapped ? b_lbo : b_sbo, d_d);
     ST_CUDA(cudaGetLastError());
     ST_CUDA(cudaDeviceSynchronize());
-    std::vector<float> d(128 * 32);
+    std::vector<float> d(128 * 96);
     ST_CUDA(cudaMemcpy(d.data(), d_d, d.size() * 4, cudaMemcpyDeviceToHost));
     double worst = 0;
     for (int r = 0; r < 128; ++r)
-      for (int n = 0; n < 32; ++n) {
+      for (int n = 0; n < 96; ++n) {
         double ref = 0;
         for (int k = 0; k < K; ++k) ref += (double)a[(size_t)(r + c.shift) * K + k] * (double)b[(size_t)n * K + k];
-        const double e = std::fabs(ref - (double)d[(size_t)r * 32 + n]);
+        const double e = std::fabs(ref - (double)d[(size_t)r * 96 + n]);
         if (!(e <= worst)) worst = std::isnan(e) ? 1e30 : e;
       }
     out[ci] = worst;
@@ -279,51 +172,12 @@ inline int run_kat(double* out, std::string* err) {
   return 0;
 }
 
-template <int M, int N, int NACC>
-inline int run_rate_one(int grid, double* cyc_per_mma, double* issue_per_mma, std::string* err) {
-  const int iters = 4096;
-  long long* d_c = nullptr;
-  ST_CUDA(cudaMalloc(&d_c, sizeof(long long) * grid * 2));
-  ST_CUDA(cudaFuncSetAttribute(umma_rate_kernel<M, N, NACC>, cudaFuncAttributeMaxDynamicSharedMemorySize, 98304 + 64));
-  umma_rate_kernel<M, N, NACC><<<grid, 128, 98304 + 64>>>(iters, d_c);   // warm-up
-  umma_rate_kernel<M, N, NACC><<<grid, 128, 98304 + 64>>>(iters, d_c);
-  ST_CUDA(cudaGetLastError());
-  ST_CUDA(cudaDeviceSynchronize());
-  std::vector<long long> c(grid * 2);
-  ST_CUDA(cudaMemcpy(c.data(), d_c, sizeof(long long) * grid * 2, cudaMemcpyDeviceToHost));
-  cudaFree(d_c);
-  long long worst = 0, worst_issue = 0;
-  for (int i = 0; i < grid; ++i) {
-    worst = std::max(worst, c[2 * i]);
-    worst_issue = std::max(worst_issue, c[2 * i + 1]);
-  }
-  *cyc_per_mma = (double)worst / iters;
-  if (issue_per_mma) *issue_per_mma = (double)worst_issue / iters;
-  return 0;
-}
-
 inline int run(int device, int variant, double* out, int n_out, std::string* err) {
   ST_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop{};
   ST_CUDA(cudaGetDeviceProperties(&prop, device));
   for (int i = 0; i < n_out; ++i) out[i] = -1.0;
   if (variant == 0) return run_kat(out, err);
-  if (variant == 1 || variant == 4) {
-    if (n_out < 16) {
-      *err = "need 16 output slots";
-      return 1;
-    }
-    const int grid = variant == 1 ? 1 : prop.multiProcessorCount;   // 4: all SMs at once (power/clock effects)
-    if (run_rate_one<128, 32, 1>(grid, &out[0], &out[8], err)) return 1;
-    if (run_rate_one<128, 32, 4>(grid, &out[1], &out[9], err)) return 1;
-    if (run_rate_one<64, 32, 4>(grid, &out[2], &out[10], err)) return 1;
-    if (run_rate_one<128, 64, 4>(grid, &out[3], &out[11], err)) return 1;
-    if (run_rate_one<128, 96, 4>(grid, &out[4], &out[12], err)) return 1;
-    if (run_rate_one<128, 128, 2>(grid, &out[5], &out[13], err)) return 1;
-    if (run_rate_one<128, 256, 2>(grid, &out[6], &out[14], err)) return 1;
-    out[7] = prop.clockRate * 1e-3;   // MHz (max)
-    return 0;
-  }
   if (variant == 2) {
     const int grid = prop.multiProcessorCount, iters = 200;
     unsigned* d_bar = nullptr;
@@ -369,39 +223,6 @@ inline int run(int device, int variant, double* out, int n_out, std::string* err
     out[1] = (double)pieces * piece;
     cudaFree(d_src);
     cudaFree(d_c);
-    return 0;
-  }
-  if (variant == 5) {
-    // out[0] = columns that changed, out[1] = first / out[2] = last changed column, out[3] = lanes that changed;
-    // out[4 + i] (i < 12): source lane now held by probe lane {0,1,2,31,32,33,63,64,65,96,126,127}[i] in the
-    // first changed column (-1: unchanged pattern not recognised)
-    if (n_out < 16) {
-      *err = "need 16 output slots";
-      return 1;
-    }
-    float* d_o = nullptr;
-    ST_CUDA(cudaMalloc(&d_o, 128 * 64 * 4));
-    ST_CUDA(cudaMemset(d_o, 0, 128 * 64 * 4));
-    tmem_shift_probe_kernel<<<1, 128>>>(0, d_o);
-    ST_CUDA(cudaGetLastError());
-    ST_CUDA(cudaDeviceSynchronize());
-    std::vector<float> o(128 * 64);
-    ST_CUDA(cudaMemcpy(o.data(), d_o, o.size() * 4, cudaMemcpyDeviceToHost));
-    cudaFree(d_o);
-    int first = -1, last = -1, ncols = 0, nlanes = 0;
-    for (int c = 0; c < 64; ++c) {
-      bool changed = false;
-      for (int l = 0; l < 128; ++l) changed |= o[(size_t)l * 64 + c] != 1000.f * c + l;
-      if (changed) {
-        if (first < 0) first = c;
-        last = c;
-        ++ncols;
-      }
-    }
-    const int probe[12] = {0, 1, 2, 31, 32, 33, 63, 64, 65, 96, 126, 127};
-    for (int l = 0; l < 128 && first >= 0; ++l) nlanes += o[(size_t)l * 64 + first] != 1000.f * first + l;
-    out[0] = ncols; out[1] = first; out[2] = last; out[3] = nlanes;
-    for (int i = 0; i < 12; ++i) out[4 + i] = first >= 0 ? (double)(o[(size_t)probe[i] * 64 + first] - 1000.f * first) : -1.0;
     return 0;
   }
   *err = "unknown selftest variant";

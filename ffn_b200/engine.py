@@ -103,7 +103,7 @@ class Engine:
     keys = ('sm_count', 'grid', 'smem_bytes', 'tiles', 'rows', 'fov_voxels', 'launches', 'last_kernel_ns')
     return dict(zip(keys, [int(v) for v in buf]))
 
-  PROFILE_SLOTS = ('barrier_wait', 'act_tma_wait', 'weight_wait', 'umma_issue', 'epi_wait_mma', 'epi_body',
+  PROFILE_SLOTS = ('barrier_wait', 'act_tma_wait', 'weight_wait', 'mma', 'unused4', 'epi_body',
                    'stage', 'paste', 'leader', 'steps', 'kernel', 'conv_layers', 'leader_policy', 'leader_pops',
                    'chain_barrier_wait', 'unused')
 

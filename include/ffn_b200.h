@@ -1,5 +1,5 @@
 /*
- * ffn_b200.h — C ABI of libffn_b200.so, the B200-native flood-filling inference engine.
+ * ffn_b200.h — C ABI of libffn_b200.so, the H100-native flood-filling inference engine.
  *
  * This is the boundary a maintainer of google/ffn binds (ctypes stub in INTEGRATION.md) to replace
  * the TensorFlow/JAX executor *and* the numpy flood-fill loop of the inference hot path.  Every
@@ -11,7 +11,7 @@
  *   - every function returns 0 on success, non-zero on failure; ffn_last_error() (thread-local)
  *     describes the failure;
  *   - calls are synchronous; one in-flight call per engine (the Python host serialises);
- *   - there is NO CPU fallback: creation fails if no sm_100 device is usable.
+ *   - there is NO CPU fallback: creation fails if no sm_90 device is usable.
  */
 #ifndef FFN_B200_H_
 #define FFN_B200_H_
@@ -27,10 +27,10 @@ typedef struct FfnCanvas FfnCanvas;
 
 /* Arithmetic of the 3x3x3 convolutions. */
 enum {
-  FFN_COMPUTE_FP16_TC = 0, /* fp16 operands, fp32 accumulate on tcgen05 tensor cores; fp32 residual stream */
+  FFN_COMPUTE_FP16_TC = 0, /* fp16 operands, fp32 accumulate on the tensor cores (wgmma); fp32 residual stream */
   FFN_COMPUTE_FP32 = 1,    /* fp32 FMA on CUDA cores ("precise" parity mode) */
   FFN_COMPUTE_FP16X2_TC = 2 /* near-fp32 on the tensor cores: every operand split into fp16 hi + lo parts,
-                             * a*w = a_hi*w_hi + a_lo*w_hi + a_hi*w_lo as three tcgen05 MMAs into the same fp32
+                             * a*w = a_hi*w_hi + a_lo*w_hi + a_hi*w_lo as three wgmma MMAs into the same fp32
                              * accumulator (weights pre-scaled by 2^10 so that w_lo stays normal) */
 };
 
@@ -128,23 +128,23 @@ int ffn_engine_set_compute_mode(FfnEngine* engine, int compute_mode);
  * object / patch at a time. */
 int ffn_engine_set_chains(FfnEngine* engine, int max_chains);
 /* Number of SMs (CTAs of the cooperative grid) this engine's kernel occupies; 0 = all.  Several engines
- * with disjoint SM budgets (e.g. 3 x 49) driven from different host threads run their persistent kernels
- * CONCURRENTLY on one GPU: the B200 form of the reference's batching across canvases
+ * with disjoint SM budgets (e.g. 3 x 44) driven from different host threads run their persistent kernels
+ * CONCURRENTLY on one GPU: the H100 form of the reference's batching across canvases
  * (InferenceRequest.batch_size / concurrent_requests, doc/manual.md:89-97). */
 int ffn_engine_set_grid(FfnEngine* engine, int num_ctas);
 /* sm count, cooperative grid size, shared memory per CTA, tiles per FoV: info[0..3]. */
 int ffn_engine_info(FfnEngine* engine, int64_t info[8]);
 
 /* Device-side cycle counters of CTA 0 (out[0..15]) and the last CTA (out[16..31]): slot 0 grid-barrier
- * wait, 1 activation TMA wait, 2 weight wait, 3 UMMA issue, 4 epilogue wait-for-MMA, 5 epilogue body,
+ * wait, 1 activation TMA wait, 2 weight wait, 3 MMAs (issue to completion), 4 unused, 5 epilogue body,
  * 6 stage, 7 paste, 8 leader, 9 steps, 10 kernel, 11 conv layers, 12-14 leader parts, 15 layer-end sync.
  * Off by default (reading the clock perturbs the critical CTA): ffn_engine_profile(e, NULL, 1) switches
  * the counters on, (e, NULL, 0) off; with out != NULL the counters are returned (and reset if reset). */
 int ffn_engine_profile(FfnEngine* engine, int64_t out[32], int reset);
 /* Tile timeline of one CTA (CTA 1) recorded while the counters are on: out[e * 2048 + i] = SM clock when event e
- * happened to that role's i-th tile since kernel start (0 producer saw the chain barrier, 1 copies issued, 2 UMMA
- * issuer saw the operands, 3 got an accumulator slot, 4 UMMAs issued, 5 epilogue saw the accumulators, 6 epilogue
- * done, 7 i-th barrier release by the signal warp); 0 = not recorded.  n <= 8 * 2048.  Debug / profiles only. */
+ * happened to that role's i-th tile since kernel start (0 producer saw the chain barrier, 1 copies issued,
+ * 2 consumers saw the operands, 4 MMAs complete, 6 epilogue done, 7 i-th barrier release by the signal warp; 3 and
+ * 5 are not recorded); 0 = not recorded.  n <= 8 * 2048.  Debug only. */
 int ffn_engine_trace(FfnEngine* engine, int64_t* out, int64_t n, int reset);
 
 /* ---- L0 drop-in: ExecutorClient.predict (ffn/inference/executor.py:134-139, 266-340) -------
@@ -233,8 +233,8 @@ int ffn_canvas_spec_stats(FfnCanvas* canvas, int64_t out[8]);
 int ffn_canvas_device_ptr(FfnCanvas* canvas, int which, void** ptr, int64_t* bytes);
 int ffn_canvas_add_id_offset(FfnCanvas* canvas, int32_t offset);
 
-/* Self tests / micro-benchmarks of the sm_100a building blocks (results in out[]; see
- * ffn_b200/csrc/selftest.cuh).  Used by tests and profiles/, not by the product path. */
+/* Self tests / micro-benchmarks of the sm_90a building blocks (results in out[]; see
+ * ffn_b200/csrc/selftest.cuh).  Used by tests, not by the product path. */
 int ffn_selftest_umma(int device, int variant, double* out, int n_out);
 
 #ifdef __cplusplus

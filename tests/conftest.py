@@ -12,7 +12,7 @@ GOLDEN = os.path.join(REPO, 'tests', 'golden')
 
 def pytest_configure(config):
   config.addinivalue_line('markers', 'slow: takes more than a few seconds on CPU')
-  config.addinivalue_line('markers', 'gpu: test needs a CUDA device (run with -m gpu on a B200)')
+  config.addinivalue_line('markers', 'gpu: test needs a CUDA device (run with -m gpu on an H100)')
 
 
 def pytest_collection_modifyitems(config, items):

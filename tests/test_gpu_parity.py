@@ -6,7 +6,7 @@ Tolerances (also stated in DESIGN.md):
                          reference golden run; qprob within +-1 LSB.
   * FFN_COMPUTE_FP16X2_TC (fp16 hi+lo split operands on the tensor cores) logits max-abs <= 1e-4 vs the
                          fp32 oracle; trajectories / labels identical to the reference golden run — the
-                         label-exact mode that runs on tcgen05.
+                         label-exact mode that runs on the tensor cores.
   * FFN_COMPUTE_FP16_TC  logits max-abs <= 4e-2 (fp16 operand rounding, fp32 accumulate; measured 3.1e-2) vs the
                          fp32 oracle and <= 1.5e-2 (measured 7.8e-3) vs the oracle with fp16-rounded conv
                          operands; flood-fill state BIT-EXACT vs the oracle
@@ -57,7 +57,7 @@ def _image(vol):
 
 
 def test_umma_descriptor_known_answer():
-  """tcgen05.mma with the K-major / no-swizzle descriptors the conv kernel uses, incl. tap shifts."""
+  """wgmma with the K-major / no-swizzle descriptors the conv kernel uses, incl. tap shifts."""
   from ffn_b200 import engine as eng
   out = eng.selftest(0, n_out=16)
   assert out[0] == 0.0 and out[1] == 0.0 and out[2] == 0.0, out   # exact: small-integer operands
@@ -137,7 +137,7 @@ def test_fp16_logits_vs_fp16_operand_oracle(engines, weights, golden_dir):
   weights rounded to fp16, fp32 accumulate).  What is left is accumulation order — which still flips
   individual fp16 roundings of the next layer's operands (1 ulp = 5e-4 relative), so two correct fp16-operand
   implementations differ by a fraction of the rounding noise itself: measured 7.8e-3 here against 3.1e-2
-  versus the fp32 oracle (B200, round 2).  A kernel error (wrong tap, wrong halo) is O(1)."""
+  versus the fp32 oracle.  A kernel error (wrong tap, wrong halo) is O(1)."""
   from oracle.network import ConvStackOracle
   w, b = weights
   pat = np.load(os.path.join(golden_dir, 'net_patches.npz'))
@@ -175,7 +175,7 @@ def test_fp16_labels_vs_fp32_reference(engines, g64):
 @pytest.mark.parametrize('mode', ['fp32', 'x2'])
 def test_fp32_segment_all_matches_reference_golden(engines, g64, mode):
   """Whole-canvas run == the reference's Canvas.segment_all on the same volume / seeds / weights, in the
-  fp32 CUDA-core mode AND in the split-fp16 tensor-core mode (label-exact on tcgen05)."""
+  fp32 CUDA-core mode AND in the split-fp16 tensor-core mode (label-exact on the tensor cores)."""
   from ffn_b200 import engine as eng
   cv = eng.DeviceCanvas(engines[mode], g64['volume'], eng.make_options(), 128.0, 33.0)
   origins, overlaps, ctr = cv.segment_all(g64['seeds'])

@@ -411,25 +411,13 @@ def test_bench_reference_arm_contract():
   assert 'workload' in d['config'] and d['data'] == 'synthetic' and d['vs_baseline'] is None
 
 
-def test_bench_traffic_comes_from_committed_ncu_capture():
-  import bench
-  t = bench.ncu_dram_traffic()
-  assert t is not None and t['steps_per_launch'] >= 16
-  # at most about the compulsory 431 KB/step (u8 image); far less when the touched part of the canvas stays in the
-  # 126 MB L2 between steps (250^3 bench canvas: 55 KB/step)
-  assert 1e4 < t['bytes_per_step'] < 431244 * 2
-
-
-def test_load_segmentation_reads_the_reference_shipped_result(tmp_path):
-  """results/fib25/sample-training2.npz of the reference checkout: a Python-2 pickle of OriginInfo under the
-  original module path — storage.load_segmentation reads it (latin1 + module mapping).  Skipped where the
-  reference checkout is absent (the GPU box)."""
+def test_load_segmentation_reads_the_reference_shipped_result(tmp_path, golden_dir):
+  """results/fib25/sample-training2.npz as shipped with the reference (stored unchanged as a fixture): a Python-2
+  pickle of OriginInfo under the original module path — storage.load_segmentation reads it (latin1 + module
+  mapping)."""
   import shutil
-  import pytest
   from ffn.inference import storage
-  src = '/root/reference/results/fib25/sample-training2.npz'
-  if not os.path.exists(src):
-    pytest.skip('reference checkout not present')
+  src = os.path.join(golden_dir, 'sample-training2.npz')
   d = tmp_path / '0' / '0'
   d.mkdir(parents=True)
   shutil.copy(src, str(d / 'seg-0_0_0.npz'))

@@ -96,17 +96,13 @@ def test_toy_flood_fill_bit_exact(golden_dir):
 
 @pytest.mark.slow
 def test_real_net_flood_fill(golden_dir):
-  """Same loop with the FIB-25 conv stack (torch CPU).  Exactness is qualified by the decision
-  margin because conv3d rounding may differ between CPUs."""
-  ckpt = os.environ.get('FFN_CKPT', '/root/reference/models/fib25/model.ckpt-27465036')
-  if not os.path.exists(ckpt + '.index'):
-    ckpt = os.path.join(golden_dir, 'fib25', 'model.ckpt-27465036')
-  if not os.path.exists(ckpt + '.index'):
-    pytest.skip('FIB-25 checkpoint not available')
+  """Same loop with the FIB-25 conv stack (torch CPU; the checkpoint's parameters as stored in
+  fib25_convstack.npz).  Exactness is qualified by the decision margin because conv3d rounding may differ
+  between CPUs."""
   from ffn_b200 import tf_checkpoint
   from oracle.network import ConvStackOracle
   g = _load(golden_dir, 'flood_fill_64.npz')
-  w, b = tf_checkpoint.load_convstack_weights(ckpt, 12)
+  w, b = tf_checkpoint.load_convstack_npz(os.path.join(golden_dir, 'fib25_convstack.npz'))
   image = (g['volume'].astype(np.float32) - 128.0) / 33.0
   canvas = ff.Canvas(ConvStackOracle(w, b), image, (33, 33, 33), (8, 8, 8), ff.Options())
   canvas.segment_all(g['seeds'])
