@@ -26,6 +26,7 @@ ARRAY_QPROB = 2
 ARRAY_IMAGE = 3
 MASK_MOVEMENT = 0
 MASK_SEED = 1
+SEED_POLICY_KINDS = {'peaks_2d': 0, 'fill_empty': 1, 'max_peaks': 2}   # FFN_SEED_*
 
 EXPORTS = [
     'ffn_last_error', 'ffn_engine_create', 'ffn_engine_destroy', 'ffn_engine_set_compute_mode', 'ffn_engine_set_chains', 'ffn_engine_set_grid',
@@ -33,7 +34,7 @@ EXPORTS = [
     'ffn_canvas_set_mask', 'ffn_canvas_segment_at', 'ffn_canvas_segment_all',
     'ffn_canvas_update_at', 'ffn_canvas_init_seed', 'ffn_canvas_read', 'ffn_canvas_write',
     'ffn_canvas_policy_state_size', 'ffn_canvas_policy_state_get', 'ffn_canvas_policy_state_set',
-    'ffn_canvas_set_resume', 'ffn_canvas_trace', 'ffn_canvas_seed_peaks', 'ffn_canvas_set_max_id', 'ffn_canvas_get_counters', 'ffn_canvas_spec_stats', 'ffn_canvas_device_ptr',
+    'ffn_canvas_set_resume', 'ffn_canvas_trace', 'ffn_canvas_seed_peaks', 'ffn_canvas_seed_policy', 'ffn_canvas_set_max_id', 'ffn_canvas_get_counters', 'ffn_canvas_spec_stats', 'ffn_canvas_device_ptr',
     'ffn_canvas_add_id_offset', 'ffn_selftest_umma',
 ]
 
@@ -63,6 +64,11 @@ class Origin(C.Structure):
 
 class Overlap(C.Structure):
   _fields_ = [('id', C.c_int32), ('other_id', C.c_int32), ('count', C.c_int64)]
+
+
+class SeedPolicyDesc(C.Structure):
+  _fields_ = [('kind', C.c_int32), ('min_distance', C.c_int32), ('threshold_abs', C.c_double),
+              ('threshold_abs_is_min', C.c_int32), ('use_threshold_rel', C.c_int32), ('threshold_rel', C.c_double)]
 
 
 class Counters(C.Structure):
@@ -127,6 +133,7 @@ def load() -> C.CDLL:
   lib.ffn_canvas_set_resume.argtypes = [p, C.c_int64, i32p, i32p]
   lib.ffn_canvas_trace.argtypes = [p, C.c_int64, p, C.POINTER(C.c_int64)]
   lib.ffn_canvas_seed_peaks.argtypes = [p, C.POINTER(C.c_float), p, p, C.c_int64, C.POINTER(C.c_int64)]
+  lib.ffn_canvas_seed_policy.argtypes = [p, C.POINTER(SeedPolicyDesc), p, p, C.c_int64, C.POINTER(C.c_int64)]
   lib.ffn_canvas_set_max_id.argtypes = [p, C.c_int64]
   lib.ffn_canvas_get_counters.argtypes = [p, C.POINTER(Counters)]
   lib.ffn_canvas_spec_stats.argtypes = [p, C.POINTER(C.c_int64)]

@@ -1272,6 +1272,99 @@ int ffn_canvas_seed_peaks(FfnCanvas* c, const float voxel_size_zyx[3], const dou
   return rc;
 }
 
+int ffn_canvas_seed_policy(FfnCanvas* c, const FfnSeedPolicyDesc* desc, const double* noise, int32_t* coords_out,
+                           int64_t cap, int64_t* n_out) {
+  if (!c || !desc || !coords_out || !n_out || cap < 1) return fail("bad argument");
+  if (desc->kind != FFN_SEED_PEAKS_2D && desc->kind != FFN_SEED_FILL_EMPTY && desc->kind != FFN_SEED_MAX_PEAKS)
+    return fail("unknown seed policy kind");
+  if (desc->min_distance < 0) return fail("min_distance must be >= 0");
+  FfnEngine* e = c->eng;
+  if (set_device(e)) return 1;
+  const CanvasDev& cv = c->cv;
+  const size_t n = c->nvox;
+  const bool is2d = desc->kind == FFN_SEED_PEAKS_2D;
+  const bool needs_edt = desc->kind != FFN_SEED_MAX_PEAKS;
+  const size_t noise_n = is2d ? (size_t)cv.sy * cv.sx : n;
+  const int blocks = e->sm_count * 16;
+  float *a = nullptr, *b = nullptr, *d = nullptr;
+  double *keys = nullptr, *m1 = nullptr, *m2 = nullptr, *d_noise = nullptr, *zbuf = nullptr, *d_w = nullptr;
+  int *vbuf = nullptr, *d_coords = nullptr;
+  unsigned long long* d_cnt = nullptr;   // [0] peaks, [1] / [2] ordered bits of the min / max key, [3] unused
+  auto cleanup = [&]() {
+    cudaFree(a); cudaFree(b); cudaFree(d); cudaFree(keys); cudaFree(m1); cudaFree(m2); cudaFree(d_noise); cudaFree(zbuf);
+    cudaFree(d_w); cudaFree(vbuf); cudaFree(d_coords); cudaFree(d_cnt);
+  };
+  // EDT scratch: 2-D sweeps only along y (lines (z, x)), 3-D also along z (lines (y, x))
+  const int maxdim = is2d ? cv.sy : std::max(cv.sz, cv.sy);
+  const size_t maxlines = is2d ? (size_t)cv.sz * cv.sx : std::max((size_t)cv.sy * cv.sx, (size_t)cv.sz * cv.sx);
+  // adaptive threshold of PolicyPeaks2d: gaussian sigma = 49/6, truncate 4 (seed.py:240-242)
+  const double sigma = 49.0 / 6.0;
+  const int radius = (int)(4.0 * sigma + 0.5);
+  std::vector<double> w(radius + 1);
+  {
+    double sum = 0;
+    for (int k = -radius; k <= radius; ++k) sum += std::exp(-0.5 / (sigma * sigma) * k * k);
+    for (int k = 0; k <= radius; ++k) w[k] = std::exp(-0.5 / (sigma * sigma) * k * k) / sum;
+  }
+  bool alloc_failed = dev_alloc(&d, n, false) || dev_alloc(&keys, n, false) || dev_alloc(&m1, n, false) ||
+                      dev_alloc(&m2, n, false) || dev_alloc(&d_coords, (size_t)cap * 3, false) || dev_alloc(&d_cnt, 4) ||
+                      (noise && dev_alloc(&d_noise, noise_n, false));
+  if (!alloc_failed && is2d)
+    alloc_failed = dev_alloc(&a, n, false) || dev_alloc(&b, n, false) || dev_alloc(&d_w, w.size(), false);
+  if (!alloc_failed && needs_edt)
+    alloc_failed = dev_alloc(&vbuf, (size_t)maxdim * maxlines, false) || dev_alloc(&zbuf, 2 * (size_t)maxdim * maxlines, false);
+  if (alloc_failed) {
+    cleanup();
+    return 1;
+  }
+  cudaStream_t st = cudaStreamPerThread;
+  const unsigned long long cnt_init[3] = {0ull, ~0ull, 0ull};
+  bool ok = cudaMemcpyAsync(d_cnt, cnt_init, sizeof(cnt_init), cudaMemcpyHostToDevice, st) == cudaSuccess;
+  if (noise) ok = ok && cudaMemcpyAsync(d_noise, noise, noise_n * sizeof(double), cudaMemcpyHostToDevice, st) == cudaSuccess;
+  if (desc->kind == FFN_SEED_PEAKS_2D) {
+    ok = ok && cudaMemcpyAsync(d_w, w.data(), w.size() * sizeof(double), cudaMemcpyHostToDevice, st) == cudaSuccess;
+    seedk::sobel_mag2d<<<blocks, 256, 0, st>>>(cv.image, cv.image_is_u8, cv.mean, cv.stddev, a, cv.sz, cv.sy, cv.sx);
+    seedk::gauss_pass<<<blocks, 256, 0, st>>>(a, b, d_w, radius, 1, cv.sz, cv.sy, cv.sx);
+    seedk::gauss_pass<<<blocks, 256, 0, st>>>(b, d, d_w, radius, 2, cv.sz, cv.sy, cv.sx);
+    // filt_edges[restrictor.mask[z]] = 1: the movement mask only (seed.py:247-250)
+    seedk::edges_kernel<<<blocks, 256, 0, st>>>(a, d, cv.mask, nullptr, d, n, d_cnt + 3);
+    seedk::edt_x<<<blocks, 128, 0, st>>>(d, cv.sz, cv.sy, cv.sx, 1.f);
+    seedk::edt_line<<<blocks, 128, 0, st>>>(d, 1, cv.sz, cv.sy, cv.sx, 1.f, vbuf, zbuf);
+    seedk::dt_finish<<<blocks, 256, 0, st>>>(d, n);
+  } else if (desc->kind == FFN_SEED_FILL_EMPTY) {
+    seedk::empty_input<<<blocks, 256, 0, st>>>(cv.seg, d, n);
+    seedk::edt_x<<<blocks, 128, 0, st>>>(d, cv.sz, cv.sy, cv.sx, 1.f);
+    seedk::edt_line<<<blocks, 128, 0, st>>>(d, 1, cv.sz, cv.sy, cv.sx, 1.f, vbuf, zbuf);
+    seedk::edt_line<<<blocks, 128, 0, st>>>(d, 0, cv.sz, cv.sy, cv.sx, 1.f, vbuf, zbuf);
+    seedk::dt_finish<<<blocks, 256, 0, st>>>(d, n);
+  } else {
+    seedk::masked_image<<<blocks, 256, 0, st>>>(cv.image, cv.image_is_u8, cv.mean, cv.stddev, cv.seg, cv.mask, cv.seed_mask, d, n);
+  }
+  const int r = desc->min_distance, rz = is2d ? 0 : r;
+  seedk::peak_keys<<<blocks, 256, 0, st>>>(d, d_noise, noise ? noise_n : 0, keys, n, d_cnt + 1);
+  seedk::box_max<<<blocks, 256, 0, st>>>(keys, m1, r, 2, cv.sz, cv.sy, cv.sx);
+  seedk::box_max<<<blocks, 256, 0, st>>>(m1, m2, r, 1, cv.sz, cv.sy, cv.sx);
+  if (rz > 0) seedk::box_max<<<blocks, 256, 0, st>>>(m2, m1, rz, 0, cv.sz, cv.sy, cv.sx);
+  seedk::peaks_select<<<blocks, 256, 0, st>>>(keys, rz > 0 ? m1 : m2, desc->threshold_abs, desc->threshold_abs_is_min,
+                                              desc->use_threshold_rel, desc->threshold_rel, d_cnt + 1, rz, r, r, cv.sz, cv.sy,
+                                              cv.sx, d_coords, (unsigned long long)cap, d_cnt);
+  unsigned long long count = 0;
+  ok = ok && cudaGetLastError() == cudaSuccess;
+  ok = ok && cudaMemcpyAsync(&count, d_cnt, sizeof(count), cudaMemcpyDeviceToHost, st) == cudaSuccess;
+  ok = ok && cudaStreamSynchronize(st) == cudaSuccess;
+  int rc = 0;
+  if (!ok) {
+    rc = fail(std::string("seed policy kernels failed: ") + cudaGetErrorString(cudaGetLastError()));
+  } else {
+    *n_out = (int64_t)count;
+    const int64_t m = std::min<int64_t>(*n_out, cap);
+    if (m > 0 && cudaMemcpy(coords_out, d_coords, (size_t)m * 3 * sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess)
+      rc = fail("seed coordinate copy failed");
+  }
+  cleanup();
+  return rc;
+}
+
 int ffn_canvas_set_max_id(FfnCanvas* c, int64_t max_id) {
   if (!c) return fail("null canvas");
   if (set_device(c->eng)) return 1;

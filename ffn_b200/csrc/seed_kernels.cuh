@@ -233,5 +233,139 @@ __global__ void peaks_kernel(const float* dt, const double* noise, int sz, int s
   }
 }
 
+// ---- PolicyPeaks2d / PolicyFillEmptySpace / PolicyMaxPeaks (seed.py:202-352) -------------------------------
+//   sobel_mag2d      9-point stencil per z-slice, reflect boundary      8 B/voxel
+//   gauss_pass x2    axes 1 and 2 only (2-D gaussian per slice)         8 B/voxel per pass
+//   edges_kernel     movement mask only (seed_mask = NULL)              9 B/voxel
+//   empty_input      seg == 0 -> EDT input                              8 B/voxel
+//   masked_image     image with excluded voxels set to 0                10-13 B/voxel
+//   edt_x, edt_line  as above (2-D: x and y sweeps only), then dt_finish 8 B/voxel
+//   peak_keys        float64 key = (double)value + noise * 1e-4, min/max 20 B/voxel (12 with a noise plane in L2)
+//   box_max x2-3     separable (2r+1) maximum of the keys, one axis each 16 B/voxel per pass
+//   peaks_select     key == box maximum, threshold, border              16 B/voxel
+
+// ndimage.generic_gradient_magnitude(slice, ndimage.sobel) on every z-slice: per in-plane axis the derivative
+// along it and [1, 2, 1] smoothing along the other, each 1-D pass stored as float32 (see sobel_mag).
+__global__ void sobel_mag2d(const void* img, int is_u8, float mean, float stddev, float* out, int sz, int sy, int sx) {
+  const size_t n = (size_t)sz * sy * sx;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int x = (int)(i % sx), y = (int)((i / sx) % sy), z = (int)(i / ((size_t)sx * sy));
+    const size_t zb = (size_t)z * sy * sx;
+    float v[3][3];
+#pragma unroll
+    for (int b = 0; b < 3; ++b) {
+      const int yy = reflect(y + b - 1, sy);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) v[b][c] = load_image(img, is_u8, mean, stddev, zb + (size_t)yy * sx + reflect(x + c - 1, sx));
+    }
+    // axis y: derivative along y, smooth along x; axis x: derivative along x, smooth along y
+    const float gy = smooth3(v[2][0] - v[0][0], v[2][1] - v[0][1], v[2][2] - v[0][2]);
+    const float gx = smooth3(v[0][2] - v[0][0], v[1][2] - v[1][0], v[2][2] - v[2][0]);
+    out[i] = sqrtf(__fadd_rn(__fmul_rn(gy, gy), __fmul_rn(gx, gx)));
+  }
+}
+
+// edt.edt(segmentation == 0): labelled voxels (including the -1 markers) are the background.
+__global__ void empty_input(const int* seg, float* d, size_t n) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+    d[i] = seg[i] == 0 ? kBig : 0.f;
+}
+
+// Squared distance -> distance; "infinite" (no background voxel on the slice / canvas) -> +inf, never a peak.
+__global__ void dt_finish(float* d, size_t n) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const float v = d[i];
+    d[i] = v >= kBig ? CUDART_INF_F : sqrtf(v);
+  }
+}
+
+// img = image.astype(float32); img[get_exclusion_mask()] = 0 (seed.py:343-345).
+__global__ void masked_image(const void* img, int is_u8, float mean, float stddev, const int* seg, const uint8_t* mask,
+                             const uint8_t* seed_mask, float* out, size_t n) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const bool excl = seg[i] > 0 || (mask && mask[i]) || (seed_mask && seed_mask[i]);
+    out[i] = excl ? 0.f : load_image(img, is_u8, mean, stddev, i);
+  }
+}
+
+// Order-preserving map of a double onto uint64, so that atomicMin / atomicMax order keys.
+__device__ __forceinline__ unsigned long long ordered_bits(double v) {
+  const unsigned long long u = (unsigned long long)__double_as_longlong(v);
+  return (u >> 63) ? ~u : (u | 0x8000000000000000ull);
+}
+__device__ __forceinline__ double from_ordered_bits(unsigned long long u) {
+  return __longlong_as_double((long long)((u >> 63) ? (u & 0x7fffffffffffffffull) : ~u));
+}
+
+// key = values + noise * 1e-4 exactly as numpy forms it (float32 -> float64, one multiply and one add, each
+// rounded to nearest; no FMA).  noise[i % noise_period] (period = Y*X for the per-slice plane, 0 = no noise).
+// minmax[0] / [1] receive the ordered bits of the minimum / maximum finite key (threshold_abs=None and
+// threshold_rel of peak_local_max).
+__global__ void peak_keys(const float* values, const double* noise, size_t noise_period, double* keys, size_t n,
+                          unsigned long long* minmax) {
+  unsigned long long lo = ~0ull, hi = 0ull;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    double k = (double)values[i];
+    if (noise_period) k = __dadd_rn(k, __dmul_rn(noise[i % noise_period], 1e-4));
+    keys[i] = k;
+    if (isfinite(k)) {
+      const unsigned long long o = ordered_bits(k);
+      lo = o < lo ? o : lo;
+      hi = o > hi ? o : hi;
+    }
+  }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) {
+    const unsigned long long l2 = __shfl_down_sync(0xffffffffu, lo, off), h2 = __shfl_down_sync(0xffffffffu, hi, off);
+    lo = l2 < lo ? l2 : lo;
+    hi = h2 > hi ? h2 : hi;
+  }
+  if ((threadIdx.x & 31) == 0 && lo <= hi) {
+    atomicMin(&minmax[0], lo);
+    atomicMax(&minmax[1], hi);
+  }
+}
+
+// One separable pass of ndimage.maximum_filter(size = 2 radius + 1, mode='nearest') along `axis`: with edge
+// clamping the window maximum is the maximum over the window's part inside the array.  Exact (max is
+// associative), so three passes equal the (2r+1)^3 box; 15 cached loads per voxel at radius 7.
+__global__ void box_max(const double* in, double* out, int radius, int axis, int sz, int sy, int sx) {
+  const size_t n = (size_t)sz * sy * sx;
+  const int len = axis == 0 ? sz : (axis == 1 ? sy : sx);
+  const size_t st = axis == 0 ? (size_t)sy * sx : (axis == 1 ? (size_t)sx : 1);
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int x = (int)(i % sx), y = (int)((i / sx) % sy), z = (int)(i / ((size_t)sx * sy));
+    const int pos = axis == 0 ? z : (axis == 1 ? y : x);
+    const int lo = max(pos - radius, 0), hi = min(pos + radius, len - 1);
+    const double* base = in + (i - (size_t)pos * st);
+    double m = base[(size_t)lo * st];
+    for (int q = lo + 1; q <= hi; ++q) m = fmax(m, base[(size_t)q * st]);
+    out[i] = m;
+  }
+}
+
+// peak_local_max by its documented definition: key == maximum of its box, key > max(threshold_abs,
+// threshold_rel * max key) (threshold_abs = the minimum key when abs_is_min), finite, and at least border[a]
+// voxels from the array border on every axis a.  Appends (z, y, x) to coords (up to cap); *count = peaks.
+__global__ void peaks_select(const double* keys, const double* boxmax, double threshold_abs, int abs_is_min, int use_rel,
+                             double threshold_rel, const unsigned long long* minmax, int bz, int by, int bx, int sz,
+                             int sy, int sx, int* coords, unsigned long long cap, unsigned long long* count) {
+  double thr = abs_is_min ? from_ordered_bits(minmax[0]) : threshold_abs;
+  if (use_rel) thr = fmax(thr, __dmul_rn(threshold_rel, from_ordered_bits(minmax[1])));
+  const size_t n = (size_t)sz * sy * sx;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const double k = keys[i];
+    if (!(isfinite(k) && k > thr && k == boxmax[i])) continue;
+    const int x = (int)(i % sx), y = (int)((i / sx) % sy), z = (int)(i / ((size_t)sx * sy));
+    if (z < bz || z >= sz - bz || y < by || y >= sy - by || x < bx || x >= sx - bx) continue;
+    const unsigned long long slot = atomicAdd(count, 1ull);
+    if (slot < cap) {
+      coords[3 * slot + 0] = z;
+      coords[3 * slot + 1] = y;
+      coords[3 * slot + 2] = x;
+    }
+  }
+}
+
 }  // namespace seedk
 }  // namespace ffn

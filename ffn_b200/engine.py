@@ -283,6 +283,41 @@ class DeviceCanvas:
     order = np.lexsort((coords[:, 2], coords[:, 1], coords[:, 0]))
     return coords[order]
 
+  def seed_policy(self, kind: str, min_distance: int, threshold_abs: Optional[float] = 0.0,
+                  threshold_rel: Optional[float] = 0.0, noise: Optional[np.ndarray] = None,
+                  cap: Optional[int] = None) -> np.ndarray:
+    """Device PolicyPeaks2d ('peaks_2d'), PolicyFillEmptySpace ('fill_empty') or PolicyMaxPeaks ('max_peaks'):
+    the raw peaks [N, 3] (z, y, x), lexicographically sorted, before the border filter of the policy.  `noise` is
+    RandomState(42).rand of shape [Y, X] for 'peaks_2d' and [Z, Y, X] otherwise; None thresholds follow
+    peak_local_max (see ffn_canvas_seed_policy)."""
+    if kind not in _lib.SEED_POLICY_KINDS:
+      raise ValueError('unknown seed policy kind %r (expected one of %s)' % (kind, sorted(_lib.SEED_POLICY_KINDS)))
+    desc = _lib.SeedPolicyDesc()
+    desc.kind = _lib.SEED_POLICY_KINDS[kind]
+    desc.min_distance = int(min_distance)
+    desc.threshold_abs_is_min = 1 if threshold_abs is None else 0
+    desc.threshold_abs = 0.0 if threshold_abs is None else float(threshold_abs)
+    desc.use_threshold_rel = 0 if threshold_rel is None else 1
+    desc.threshold_rel = 0.0 if threshold_rel is None else float(threshold_rel)
+    nz = None
+    if noise is not None:
+      nz = np.ascontiguousarray(noise, dtype=np.float64)
+      want = self.shape[1:] if kind == 'peaks_2d' else self.shape
+      if nz.shape != want:
+        raise ValueError('noise shape %r, expected %r' % (nz.shape, want))
+    cap = int(cap or max(self.shape[0] * self.shape[1] * self.shape[2] // 64, 4096))
+    while True:
+      out = np.empty((cap, 3), dtype=np.int32)
+      n = C.c_int64(0)
+      _lib.check(self._lib.ffn_canvas_seed_policy(self._h, C.byref(desc), _lib.ptr(nz) if nz is not None else None,
+                                                   _lib.ptr(out), cap, C.byref(n)))
+      if n.value <= cap:
+        break
+      cap = int(n.value)
+    coords = out[:n.value]
+    order = np.lexsort((coords[:, 2], coords[:, 1], coords[:, 0]))
+    return coords[order]
+
   def set_max_id(self, max_id: int):
     _lib.check(self._lib.ffn_canvas_set_max_id(self._h, int(max_id)))
 

@@ -1,9 +1,18 @@
-"""Seed policies: iterators over (z, y, x) starting points, computed once per canvas on the host.
+"""Seed policies: iterators over (z, y, x) starting points, computed once per canvas.
 
 Mirrors ffn/inference/seed.py: `BaseSeedPolicy` (:37-130, incl. the border filter :81-88 and the
-checkpoint state :100-113), `PolicyPeaks` (:142-199), `PolicyMax` (:307-313), `PolicyGrid3d`
-(:411-430), `PolicyGrid2d` (:433-452), `PolicyInvertOrigins` (:455-469), `PolicyDenseSeeds`
-(:472-492), `ReverseCoords` (:495-504), `SequentialPolicies` (:507-544).
+checkpoint state :100-113), `PolicyPeaks` (:142-199), `PolicyPeaks2d` (:202-280), `PolicyFillEmptySpace`
+(:283-304), `PolicyMax` (:307-313), `PolicyMaxPeaks` (:316-352), `PolicyGrid3d` (:411-430), `PolicyGrid2d`
+(:433-452), `PolicyInvertOrigins` (:455-469), `PolicyDenseSeeds` (:472-492), `ReverseCoords` (:495-504),
+`SequentialPolicies` (:507-544).  `PolicyImagePeaks3D2D` and `PolicyImagePeaks2DDisk` are not provided: they
+add no tie-break noise, so their output on real images depends on how skimage orders and spaces equal-valued
+peaks.
+
+`PolicyPeaks`, `PolicyPeaks2d`, `PolicyFillEmptySpace` and `PolicyMaxPeaks` run on the device when the canvas
+has one (the image, segmentation and masks are resident there; only the RandomState(42) tie-break noise is
+uploaded), and otherwise with scipy on the host; both paths yield the same list.  PolicyPeaks2d / FillEmptySpace
+define one case the reference leaves to the `edt` package: with no finite distance (a slice without an edge
+voxel, a canvas without a labelled voxel) there are no seeds.
 
 `PolicyPeaks` depends upstream on `edt.edt` and `skimage.feature.peak_local_max`, neither of
 which is installable offline; it is restated with scipy (exact Euclidean distance transform with
@@ -166,6 +175,118 @@ def _distance_map(is_edge, voxel_size_zyx, excluded):
   dist = ndimage.distance_transform_edt(~is_edge, sampling=voxel_size_zyx).astype(np.float32)
   dist[excluded | ~np.isfinite(dist)] = -1
   return dist
+
+
+def _device_canvas(canvas, uses_movement_mask):
+  """The canvas' DeviceCanvas when a policy may run there, else None.  The device's movement mask also
+  carries the shift-mask rule, which the reference's policies do not apply: a policy that reads
+  `restrictor.mask` runs on the host when a shift mask is set."""
+  dev = getattr(canvas, '_dev', None)
+  if dev is not None and uses_movement_mask and getattr(canvas.restrictor, 'shift_mask', None) is not None:
+    return None
+  return dev
+
+
+def _local_peaks(keys, min_distance, threshold_abs, threshold_rel):
+  """skimage.feature.peak_local_max(keys, min_distance, threshold_abs, threshold_rel) by its documented
+  definition: a voxel is a peak iff it equals the maximum of its (2 min_distance + 1)^ndim neighbourhood
+  (edges clamped), exceeds max(threshold_abs, threshold_rel * max) (threshold_abs None: the minimum) and lies
+  at least min_distance from the border on every axis.  Non-finite keys are never peaks and do not enter the
+  minimum / maximum.  Returns the peak indices in C order."""
+  finite = np.isfinite(keys)
+  if not finite.any():
+    return np.zeros((0, keys.ndim), dtype=np.int64)
+  thr = float(keys[finite].min()) if threshold_abs is None else float(threshold_abs)
+  if threshold_rel is not None:
+    thr = max(thr, float(threshold_rel) * float(keys[finite].max()))
+  size = 2 * min_distance + 1
+  peak = (keys == ndimage.maximum_filter(keys, size=size, mode='nearest')) & (keys > thr) & finite
+  inner = np.zeros(keys.shape, dtype=bool)
+  inner[tuple(slice(min_distance, s - min_distance) for s in keys.shape)] = True
+  return np.argwhere(peak & inner)
+
+
+class PolicyPeaks2d(BaseSeedPolicy):
+  """Per z-slice: 2-D Sobel edges -> adaptive threshold -> 2-D distance transform -> local maxima
+  (seed.py:202-280).  Only the movement mask counts as edges; seeds in labelled or seed-masked voxels are
+  proposed and rejected later by the canvas, as in the reference.  A slice without any edge voxel has no
+  finite distance and yields no seeds."""
+
+  def __init__(self, canvas, min_distance=7, threshold_abs=2.5, sort_cmp='ascending', **kwargs):
+    super().__init__(canvas, **kwargs)
+    self.min_distance = min_distance
+    self.threshold_abs = threshold_abs
+    self.sort_reverse = sort_cmp.strip().lower().startswith('de')
+
+  def init_coords(self):
+    shape = tuple(int(v) for v in self.canvas.shape)
+    noise = _tie_break_noise(shape[1:])     # every slice draws the same RandomState(42) plane
+    dev = _device_canvas(self.canvas, uses_movement_mask=True)
+    if dev is not None:
+      with self.canvas._exec_client.engine_lock:         # pylint: disable=protected-access
+        coords = dev.seed_policy('peaks_2d', self.min_distance, self.threshold_abs, 0, noise)
+    else:
+      image = np.asarray(self.canvas.image)
+      mask = getattr(self.canvas.restrictor, 'mask', None)
+      chunks = []
+      for z in range(shape[0]):
+        is_edge = _edge_mask(image[z], None)
+        if mask is not None:
+          is_edge |= np.asarray(mask[z]).astype(bool)
+        if not is_edge.any():
+          continue
+        dt = ndimage.distance_transform_edt(~is_edge).astype(np.float32)
+        idx = _local_peaks(dt + noise * 1e-4, self.min_distance, self.threshold_abs, 0)
+        chunks.append(np.concatenate([np.full((idx.shape[0], 1), z, dtype=np.int64), idx], axis=1))
+      coords = np.concatenate(chunks, axis=0) if chunks else np.zeros((0, 3), dtype=np.int64)
+    self.coords = np.array(sorted(map(tuple, np.asarray(coords).astype(int).tolist()),
+                                  reverse=self.sort_reverse)).reshape(-1, 3)
+
+
+class PolicyFillEmptySpace(BaseSeedPolicy):
+  """Local maxima of the distance transform of the unlabelled voxels (seed.py:283-304): seeds for the gaps
+  of an existing segmentation (init_segmentation, or an earlier policy of SequentialPolicies).  The -1
+  markers count as labelled.  A canvas without any labelled voxel yields no seeds."""
+
+  def init_coords(self):
+    shape = tuple(int(v) for v in self.canvas.shape)
+    noise = _tie_break_noise(shape)
+    dev = _device_canvas(self.canvas, uses_movement_mask=False)
+    if dev is not None:
+      with self.canvas._exec_client.engine_lock:         # pylint: disable=protected-access
+        coords = dev.seed_policy('fill_empty', 2, 0.5, 0, noise)
+    else:
+      empty = np.asarray(self.canvas.segmentation) == 0
+      if empty.all():
+        coords = np.zeros((0, 3), dtype=np.int64)
+      else:
+        dt = ndimage.distance_transform_edt(empty).astype(np.float32)
+        coords = _local_peaks(dt + noise * 1e-4, 2, 0.5, 0)
+    self.coords = np.array(sorted(map(tuple, np.asarray(coords).astype(int).tolist()))).reshape(-1, 3)
+
+
+class PolicyMaxPeaks(BaseSeedPolicy):
+  """Local maxima of the image intensity with the excluded voxels (labels, movement mask, seed mask) set to 0
+  (seed.py:316-352)."""
+
+  def __init__(self, canvas, min_distance=3, threshold_abs=0, threshold_rel=0, **kwargs):
+    super().__init__(canvas, **kwargs)
+    self.min_distance = min_distance
+    self.threshold_abs = threshold_abs
+    self.threshold_rel = threshold_rel
+
+  def init_coords(self):
+    shape = tuple(int(v) for v in self.canvas.shape)
+    noise = _tie_break_noise(shape)
+    dev = _device_canvas(self.canvas, uses_movement_mask=True)
+    if dev is not None:
+      with self.canvas._exec_client.engine_lock:         # pylint: disable=protected-access
+        coords = dev.seed_policy('max_peaks', self.min_distance, self.threshold_abs, self.threshold_rel, noise)
+    else:
+      img = np.asarray(self.canvas.image).astype(np.float32)
+      img[self.get_exclusion_mask()] = 0
+      coords = _local_peaks(img + noise * 1e-4, self.min_distance, self.threshold_abs, self.threshold_rel)
+    self.coords = np.array(sorted(map(tuple, np.asarray(coords).astype(int).tolist()))).reshape(-1, 3)
 
 
 class PolicyMax(BaseSeedPolicy):

@@ -218,6 +218,29 @@ int ffn_canvas_trace(FfnCanvas* canvas, int64_t capacity, int32_t* events_out, i
  * (z, y, x) triples in arbitrary order (sort them for the policy); *n_out = number of peaks found. */
 int ffn_canvas_seed_peaks(FfnCanvas* canvas, const float voxel_size_zyx[3], const double* noise,
                           int32_t* coords_out, int64_t cap, int64_t* n_out);
+
+/* Seed policies built on peak_local_max (ffn/inference/seed.py:133-139, 202-352). */
+enum {
+  FFN_SEED_PEAKS_2D = 0,   /* PolicyPeaks2d: per z-slice 2-D Sobel -> gaussian(sigma 49/6) threshold, movement mask as
+                            * edges -> unit-spacing 2-D EDT; peaks within each slice; noise [Y,X] */
+  FFN_SEED_FILL_EMPTY = 1, /* PolicyFillEmptySpace: 3-D EDT of segmentation == 0; noise [Z,Y,X] */
+  FFN_SEED_MAX_PEAKS = 2   /* PolicyMaxPeaks: image with labels > 0 | movement mask | seed mask set to 0; noise [Z,Y,X] */
+};
+typedef struct {
+  int32_t kind;                 /* FFN_SEED_* */
+  int32_t min_distance;         /* neighbourhood radius and border exclusion (y, x; and z unless PEAKS_2D) */
+  double threshold_abs;
+  int32_t threshold_abs_is_min; /* threshold_abs=None: the minimum key */
+  int32_t use_threshold_rel;    /* 0: threshold_rel=None */
+  double threshold_rel;         /* threshold = max(threshold_abs, threshold_rel * maximum key) */
+} FfnSeedPolicyDesc;
+/* The peaks of one of the policies above on the canvas' resident image, segmentation and masks: voxels whose
+ * key (double)value + noise * 1e-4 (noise: host float64 = RandomState(42).rand, or NULL) equals the maximum of
+ * its (2 min_distance + 1)-box (edges clamped), exceeds the threshold and lies min_distance or more from the
+ * border.  A slice (PEAKS_2D) or canvas (FILL_EMPTY) without any background voxel for the distance transform
+ * has no finite distance and yields no peaks.  coords_out / cap / *n_out as for ffn_canvas_seed_peaks. */
+int ffn_canvas_seed_policy(FfnCanvas* canvas, const FfnSeedPolicyDesc* desc, const double* noise,
+                           int32_t* coords_out, int64_t cap, int64_t* n_out);
 /* Canvas._max_id / counters carried across calls (checkpoint restore, init segmentation). */
 int ffn_canvas_set_max_id(FfnCanvas* canvas, int64_t max_id);
 int ffn_canvas_get_counters(FfnCanvas* canvas, FfnCounters* out);
