@@ -35,7 +35,7 @@ EXPORTS = [
     'ffn_canvas_update_at', 'ffn_canvas_init_seed', 'ffn_canvas_read', 'ffn_canvas_write',
     'ffn_canvas_policy_state_size', 'ffn_canvas_policy_state_get', 'ffn_canvas_policy_state_set',
     'ffn_canvas_set_resume', 'ffn_canvas_trace', 'ffn_canvas_seed_peaks', 'ffn_canvas_seed_policy', 'ffn_canvas_set_max_id', 'ffn_canvas_get_counters', 'ffn_canvas_spec_stats', 'ffn_canvas_device_ptr',
-    'ffn_canvas_add_id_offset', 'ffn_selftest_umma',
+    'ffn_canvas_add_id_offset', 'ffn_decision_points', 'ffn_selftest_umma',
 ]
 
 
@@ -69,6 +69,16 @@ class Overlap(C.Structure):
 class SeedPolicyDesc(C.Structure):
   _fields_ = [('kind', C.c_int32), ('min_distance', C.c_int32), ('threshold_abs', C.c_double),
               ('threshold_abs_is_min', C.c_int32), ('use_threshold_rel', C.c_int32), ('threshold_rel', C.c_double)]
+
+
+class DecisionPointDesc(C.Structure):
+  _fields_ = [('shape_zyx', C.c_int32 * 3), ('voxel_size_xyz', C.c_int32 * 3), ('use_max_distance', C.c_int32),
+              ('reserved', C.c_int32), ('max_distance', C.c_double), ('box_start_zyx', C.c_int32 * 3),
+              ('box_size_zyx', C.c_int32 * 3), ('dust_threshold', C.c_int64)]
+
+
+# FfnDecisionPoint, as a numpy record so that the output array is filled in place
+DECISION_POINT_DTYPE = np.dtype([('id_a', '<u8'), ('id_b', '<u8'), ('dist', '<f8'), ('point_xyz', '<i8', (3,))])
 
 
 class Counters(C.Structure):
@@ -139,6 +149,7 @@ def load() -> C.CDLL:
   lib.ffn_canvas_spec_stats.argtypes = [p, C.POINTER(C.c_int64)]
   lib.ffn_canvas_device_ptr.argtypes = [p, C.c_int, C.POINTER(p), C.POINTER(C.c_int64)]
   lib.ffn_canvas_add_id_offset.argtypes = [p, C.c_int32]
+  lib.ffn_decision_points.argtypes = [C.c_int, C.POINTER(DecisionPointDesc), p, p, C.c_int64, C.POINTER(C.c_int64)]
   lib.ffn_selftest_umma.argtypes = [C.c_int, C.c_int, C.POINTER(C.c_double), C.c_int]
   for name in EXPORTS:
     if name not in ('ffn_last_error', 'ffn_engine_destroy', 'ffn_canvas_destroy'):

@@ -23,7 +23,10 @@
 #undef FFN_KNS
 #undef FFN_PROFILE
 #include "seed_kernels.cuh"
+#include "decision_kernels.cuh"
 #include "selftest.cuh"
+
+#include <cub/cub.cuh>
 
 namespace {
 
@@ -114,6 +117,35 @@ using namespace ffn;
 
 int set_device(const FfnEngine* e) {
   CUDA_OK(cudaSetDevice(e->device));
+  return 0;
+}
+
+// Device allocations of one call, released on every return path.
+struct DevBufs {
+  std::vector<void*> p;
+  ~DevBufs() { for (void* q : p) cudaFree(q); }
+  template <typename T>
+  int get(T** out, size_t count) {
+    if (dev_alloc(out, count, false)) return 1;
+    p.push_back(*out);
+    return 0;
+  }
+  void release(void* q) {
+    p.erase(std::remove(p.begin(), p.end(), q), p.end());
+    cudaFree(q);
+  }
+};
+
+// The library only contains sm_90a code: every entry point that takes a device index accepts an sm_90 device only.
+int check_device(int device, cudaDeviceProp* prop) {
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
+    return fail("no CUDA device: libffn_b200 has no CPU fallback");
+  if (device < 0 || device >= ndev) return fail("bad device index");
+  CUDA_OK(cudaGetDeviceProperties(prop, device));
+  if (prop->major != 9 || prop->minor != 0)
+    return fail(std::string("device is sm_") + std::to_string(prop->major) + std::to_string(prop->minor) +
+                "; this library only contains sm_90a code");
   return 0;
 }
 
@@ -371,15 +403,8 @@ int ffn_engine_create(int device, const FfnModelDesc* model, const float* const*
     if (model->deltas_zyx[k] < 0 || model->deltas_zyx[k] > model->fov_zyx[k] / 2)
       return fail("deltas must lie in [0, fov // 2]");
   }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
-    return fail("no CUDA device: libffn_b200 has no CPU fallback");
-  if (device < 0 || device >= ndev) return fail("bad device index");
   cudaDeviceProp prop{};
-  CUDA_OK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 9 || prop.minor != 0)
-    return fail(std::string("device is sm_") + std::to_string(prop.major) + std::to_string(prop.minor) +
-                "; this library only contains sm_90a code");
+  if (check_device(device, &prop)) return 1;
   std::unique_ptr<FfnEngine> e(new FfnEngine());
   e->device = device;
   CUDA_OK(cudaSetDevice(device));
@@ -1408,6 +1433,157 @@ int ffn_canvas_add_id_offset(FfnCanvas* c, int32_t offset) {
   relabel_offset_kernel<<<c->eng->sm_count * 8, 256, 0, cudaStreamPerThread>>>(c->cv.seg, c->nvox, offset);
   CUDA_OK(cudaGetLastError());
   CUDA_OK(cudaStreamSynchronize(cudaStreamPerThread));
+  return 0;
+}
+
+int ffn_decision_points(int device, const FfnDecisionPointDesc* desc, uint64_t* labels, FfnDecisionPoint* out,
+                        int64_t cap, int64_t* n_out) {
+  using dpk::u64;
+  if (!desc || !labels || !n_out || cap < 0 || (cap > 0 && !out)) return fail("bad argument");
+  const int sz = desc->shape_zyx[0], sy = desc->shape_zyx[1], sx = desc->shape_zyx[2];
+  if (sz < 1 || sy < 1 || sx < 1) return fail("shape must be positive");
+  const size_t n = (size_t)sz * sy * sx;
+  if (n >= (1ull << 31)) return fail("decision points support volumes of fewer than 2^31 voxels");
+  const int w[3] = {desc->voxel_size_xyz[2], desc->voxel_size_xyz[1], desc->voxel_size_xyz[0]};   // z, y, x
+  for (int a = 0; a < 3; ++a) {
+    if (w[a] < 1) return fail("voxel sizes must be positive integers");
+    if (desc->box_start_zyx[a] < 0 || desc->box_size_zyx[a] < 0 ||
+        (int64_t)desc->box_start_zyx[a] + desc->box_size_zyx[a] > desc->shape_zyx[a])
+      return fail("subvolume box lies outside the volume");
+  }
+  cudaDeviceProp prop{};
+  if (check_device(device, &prop)) return 1;
+  CUDA_OK(cudaSetDevice(device));
+  cudaStream_t st = cudaStreamPerThread;
+  const int blocks = prop.multiProcessorCount * 16;
+  DevBufs bufs;
+
+  // Compaction: sorted unique ids and their counts; the kept ids (non-zero, not dust) in uint64 order.
+  u64 *d_lab = nullptr, *d_sorted = nullptr, *d_unique = nullptr, *d_kept = nullptr;
+  unsigned* d_counts = nullptr;
+  unsigned char* d_flags = nullptr;
+  int* d_num = nullptr;   // [0] runs, [1] kept ids
+  char* d_temp = nullptr;
+  if (bufs.get(&d_lab, n) || bufs.get(&d_sorted, n) || bufs.get(&d_unique, n) || bufs.get(&d_counts, n) ||
+      bufs.get(&d_num, 2))
+    return 1;
+  size_t tb_sort = 0, tb_rle = 0, tb_sel = 0;
+  CUDA_OK(cub::DeviceRadixSort::SortKeys(nullptr, tb_sort, d_lab, d_sorted, (int)n, 0, 64, st));
+  CUDA_OK(cub::DeviceRunLengthEncode::Encode(nullptr, tb_rle, d_sorted, d_unique, d_counts, d_num, (int)n, st));
+  CUDA_OK(cub::DeviceSelect::Flagged(nullptr, tb_sel, d_unique, d_flags, d_sorted, d_num + 1, (int)n, st));
+  if (bufs.get(&d_temp, std::max(tb_sort, std::max(tb_rle, tb_sel)))) return 1;
+  CUDA_OK(cudaMemcpyAsync(d_lab, labels, n * sizeof(u64), cudaMemcpyHostToDevice, st));
+  CUDA_OK(cub::DeviceRadixSort::SortKeys(d_temp, tb_sort, d_lab, d_sorted, (int)n, 0, 64, st));
+  CUDA_OK(cub::DeviceRunLengthEncode::Encode(d_temp, tb_rle, d_sorted, d_unique, d_counts, d_num, (int)n, st));
+  int nruns = 0;
+  u64 first_id = 0;
+  CUDA_OK(cudaMemcpyAsync(&nruns, d_num, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaMemcpyAsync(&first_id, d_unique, sizeof(u64), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+  if (bufs.get(&d_flags, nruns)) return 1;
+  dpk::flag_kept<<<blocks, 256, 0, st>>>(d_unique, d_counts, nruns, desc->dust_threshold, d_flags);
+  d_kept = d_sorted;   // the sorted copy is no longer needed
+  CUDA_OK(cub::DeviceSelect::Flagged(d_temp, tb_sel, d_unique, d_flags, d_kept, d_num + 1, nruns, st));
+  int nkept = 0;
+  CUDA_OK(cudaMemcpyAsync(&nkept, d_num + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+  bufs.release(d_unique);
+  bufs.release(d_counts);
+  bufs.release(d_temp);
+  bufs.release(d_flags);
+  const bool dust_cleared = nkept < nruns - (first_id == 0 ? 1 : 0);
+
+  // Key range: every finite key (D + 1) * M - 1 must stay below kInf.
+  int log_m = 0;
+  while ((1ull << log_m) <= (u64)nkept) ++log_m;
+  const u64 m = 1ull << log_m;
+  unsigned __int128 dmax = 0;
+  for (int a = 0; a < 3; ++a) {
+    const unsigned __int128 e = (unsigned __int128)w[a] * (unsigned __int128)(desc->shape_zyx[a] - 1);
+    dmax += e * e;
+  }
+  if (dmax >= ((unsigned __int128)1 << 64) || ((dmax + 1) << log_m) >= ((unsigned __int128)1 << 64))
+    return fail("voxel size and extent too large for exact 64-bit distance keys: (D_max + 1) * M = (" +
+                std::to_string((double)dmax) + " + 1) * " + std::to_string(m) + " does not fit in 64 bits");
+
+  u64 *keys = nullptr, *keys2 = nullptr;
+  if (bufs.get(&keys, n)) return 1;
+  dpk::init_keys<<<blocks, 256, 0, st>>>(d_lab, d_kept, nkept, keys, n);
+  CUDA_OK(cudaGetLastError());
+  if (dust_cleared) CUDA_OK(cudaMemcpyAsync(labels, d_lab, n * sizeof(u64), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+  bufs.release(d_lab);
+  *n_out = 0;
+  dpk::PairGeom g{};
+  for (int a = 0; a < 3; ++a) {
+    g.lo[a] = desc->box_start_zyx[a];
+    g.size[a] = desc->box_size_zyx[a];
+  }
+  if (nkept == 0 || (size_t)g.size[0] * g.size[1] * g.size[2] == 0) return 0;
+
+  // Exact nearest-id transform: x sweeps in place, then y (keys -> keys2) and z (keys2 -> keys).
+  int *sbuf = nullptr, *tbuf = nullptr;
+  if (bufs.get(&keys2, n) || bufs.get(&sbuf, n) || bufs.get(&tbuf, n)) return 1;
+  dpk::nid_x<<<blocks, 128, 0, st>>>(keys, sz, sy, sx, m * (u64)w[2] * (u64)w[2], m);
+  dpk::nid_line<<<blocks, 128, 0, st>>>(keys, keys2, 1, sz, sy, sx, m * (u64)w[1] * (u64)w[1], sbuf, tbuf);
+  dpk::nid_line<<<blocks, 128, 0, st>>>(keys2, keys, 0, sz, sy, sx, m * (u64)w[0] * (u64)w[0], sbuf, tbuf);
+  CUDA_OK(cudaGetLastError());
+  CUDA_OK(cudaStreamSynchronize(st));
+  bufs.release(keys2);
+  bufs.release(sbuf);
+  bufs.release(tbuf);
+
+  // Pair search; a table that fills up is discarded and rebuilt four times larger.
+  g.sy = sy;
+  g.sx = sx;
+  g.m = m;
+  g.log_m = log_m;
+  g.use_max_distance = desc->use_max_distance;
+  g.max_distance = desc->max_distance;
+  dpk::PairTable t{};
+  u64* tmem = nullptr;
+  u64* d_misc = nullptr;   // [0] reserved slots, [1] overflow flag, [2] emitted pairs
+  if (bufs.get(&d_misc, 3)) return 1;
+  for (u64 tcap = 4096;; tcap *= 4) {
+    if (bufs.get(&tmem, 8 * tcap)) return 1;
+    t.key = tmem;
+    t.dist = tmem + tcap;
+    t.cnt = tmem + 2 * tcap;
+    t.sum = tmem + 3 * tcap;
+    t.c2 = tmem + 6 * tcap;
+    t.ord = tmem + 7 * tcap;
+    t.cap = tcap;
+    t.limit = tcap / 2;
+    t.used = d_misc;
+    t.overflow = (int*)(d_misc + 1);
+    CUDA_OK(cudaMemsetAsync(d_misc, 0, 3 * sizeof(u64), st));
+    dpk::table_init<<<blocks, 256, 0, st>>>(t);
+    dpk::pair_pass<1><<<blocks, 256, 0, st>>>(keys, g, t);
+    CUDA_OK(cudaGetLastError());
+    u64 misc[2] = {0, 0};
+    CUDA_OK(cudaMemcpyAsync(misc, d_misc, sizeof(misc), cudaMemcpyDeviceToHost, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    if (misc[1] == 0) break;
+    bufs.release(tmem);
+  }
+  dpk::pair_pass<2><<<blocks, 256, 0, st>>>(keys, g, t);
+  dpk::pair_pass<3><<<blocks, 256, 0, st>>>(keys, g, t);
+  dpk::pair_pass<4><<<blocks, 256, 0, st>>>(keys, g, t);
+  FfnDecisionPoint* d_out = nullptr;
+  if (bufs.get(&d_out, t.limit)) return 1;
+  dpk::emit_pairs<<<blocks, 256, 0, st>>>(t, d_kept, g.size[1], g.size[2], d_out, d_misc + 2);
+  CUDA_OK(cudaGetLastError());
+  u64 npairs = 0;
+  CUDA_OK(cudaMemcpyAsync(&npairs, d_misc + 2, sizeof(u64), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+  std::vector<FfnDecisionPoint> host(npairs);
+  CUDA_OK(cudaMemcpyAsync(host.data(), d_out, npairs * sizeof(FfnDecisionPoint), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+  std::sort(host.begin(), host.end(), [](const FfnDecisionPoint& p, const FfnDecisionPoint& q) {
+    return p.id_a < q.id_a || (p.id_a == q.id_a && p.id_b < q.id_b);
+  });
+  *n_out = (int64_t)npairs;
+  std::copy(host.begin(), host.begin() + std::min<int64_t>(cap, (int64_t)npairs), out);
   return 0;
 }
 

@@ -256,6 +256,34 @@ int ffn_canvas_spec_stats(FfnCanvas* canvas, int64_t out[8]);
 int ffn_canvas_device_ptr(FfnCanvas* canvas, int which, void** ptr, int64_t* bytes);
 int ffn_canvas_add_id_offset(FfnCanvas* canvas, int32_t offset);
 
+/* ---- decision points: find_decision_points (ffn/utils/decision_point.py:27-145) ---------------------------------
+ * Every empty voxel takes the id of the nearest labelled voxel (exact squared physical distance; the smallest id
+ * on ties), unless that distance exceeds max_distance.  Within the box, every pair of different ids (a < b) that
+ * then touch under one of the 7 offsets of itertools.product((0,-1),(0,-1),(0,-1)) gets the minimal
+ * dist = (edt_a + edt_b) / 2 and, among the rows at that minimum, the one closest to their centroid (first in
+ * (offset, raster) order on ties). */
+typedef struct {
+  int32_t shape_zyx[3];
+  int32_t voxel_size_xyz[3];  /* positive integers */
+  int32_t use_max_distance;   /* 0: max_distance=None */
+  int32_t reserved;
+  double max_distance;
+  int32_t box_start_zyx[3];   /* subvol_box; the whole volume when it is not given */
+  int32_t box_size_zyx[3];
+  int64_t dust_threshold;     /* > 0: clear_dust first, ids with fewer voxels become 0 (optimize_sparse) */
+} FfnDecisionPointDesc;
+typedef struct {
+  uint64_t id_a, id_b;        /* id_a < id_b */
+  double dist;
+  int64_t point_xyz[3];       /* relative to the box */
+} FfnDecisionPoint;
+/* labels: host uint64 [Z,Y,X]; written back (dust cleared) only when dust_threshold removed an id.  out receives the
+ * first min(count, cap) decision points in (id_a, id_b) order; *n_out = count.  Fails, with no approximate answer,
+ * when (D_max + 1) * M does not fit in 64 bits (D_max: the largest squared physical distance in the volume, M: the
+ * power of two above the number of ids). */
+int ffn_decision_points(int device, const FfnDecisionPointDesc* desc, uint64_t* labels, FfnDecisionPoint* out,
+                        int64_t cap, int64_t* n_out);
+
 /* Self tests / micro-benchmarks of the sm_90a building blocks (results in out[]; see
  * ffn_b200/csrc/selftest.cuh).  Used by tests, not by the product path. */
 int ffn_selftest_umma(int device, int variant, double* out, int n_out);
