@@ -190,6 +190,16 @@ Geom make_geom(const FfnModelDesc& m) {
 // How many chains a launch may use.
 int chain_limit(const FfnEngine* e) { return std::max(1, std::min(e->max_chains, (int)kMaxChains)); }
 
+// The flood kernel instances: {plain, profiled} x {fp16 / fp32, split fp16}.
+const void* const kFloodKernels[2][2] = {
+    {reinterpret_cast<const void*>(plain::ffn_flood_kernel<false>), reinterpret_cast<const void*>(plain::ffn_flood_kernel<true>)},
+    {reinterpret_cast<const void*>(profiled::ffn_flood_kernel<false>),
+     reinterpret_cast<const void*>(profiled::ffn_flood_kernel<true>)}};
+
+const void* flood_kernel(const FfnEngine* e) {
+  return kFloodKernels[e->profiling ? 1 : 0][e->compute_mode == FFN_COMPUTE_FP16X2_TC ? 1 : 0];
+}
+
 // Launches the persistent kernel once and waits for it.  `c` may be null (predict).
 int launch(FfnEngine* e, FfnCanvas* c, int nchains, const Job& job) {
   KParams p{};
@@ -224,9 +234,8 @@ int launch(FfnEngine* e, FfnCanvas* c, int nchains, const Job& job) {
   for (int k = 0; k < kMaxChains; ++k) CUDA_OK(cudaMemsetAsync(e->cws[k].bar, 0, sizeof(unsigned), cudaStreamPerThread));
   void* args[] = {&p};
   CUDA_OK(cudaEventRecord(e->ev0, cudaStreamPerThread));
-  CUDA_OK(cudaLaunchCooperativeKernel(e->profiling ? reinterpret_cast<const void*>(profiled::ffn_flood_kernel)
-                                                   : reinterpret_cast<const void*>(plain::ffn_flood_kernel), dim3(e->grid),
-                                      dim3(kThreads), args, (size_t)e->smem_bytes, cudaStreamPerThread));
+  CUDA_OK(cudaLaunchCooperativeKernel(flood_kernel(e), dim3(e->grid), dim3(kThreads), args, (size_t)e->smem_bytes,
+                                      cudaStreamPerThread));
   CUDA_OK(cudaEventRecord(e->ev1, cudaStreamPerThread));
   CUDA_OK(cudaStreamSynchronize(cudaStreamPerThread));
   float ms = 0.f;
@@ -428,11 +437,13 @@ int ffn_engine_create(int device, const FfnModelDesc* model, const float* const*
   e->smem_bytes = L.total;
   if ((size_t)L.total > prop.sharedMemPerBlockOptin)
     return fail("field of view too large for the shared-memory operand staging");
-  CUDA_OK(cudaFuncSetAttribute(plain::ffn_flood_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total));
-  CUDA_OK(cudaFuncSetAttribute(profiled::ffn_flood_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total));
-  int per_sm = 0;
-  CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, plain::ffn_flood_kernel, kThreads, L.total));
-  if (per_sm < 1) return fail("persistent kernel does not fit on an SM");
+  for (const auto& by_mode : kFloodKernels)
+    for (const void* k : by_mode) {
+      CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total));
+      int per_sm = 0;
+      CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, kThreads, L.total));
+      if (per_sm < 1) return fail("persistent kernel does not fit on an SM");
+    }
   e->grid = std::min(e->sm_count, g.nt);
   if ((g.nt + e->grid - 1) / e->grid > kMaxTilesPerCta)
     return fail("field of view needs more than " + std::to_string(kMaxTilesPerCta) + " tiles per SM");

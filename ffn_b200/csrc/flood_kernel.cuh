@@ -44,7 +44,7 @@ namespace FFN_KNS {
 struct Ctx {
   const KParams* p;
   int tid, warp, lane, cta, G;
-  int t_begin, t_end;          // tiles owned by this CTA
+  int t_begin, t_end;          // tiles whose rows this CTA stages and pastes (parity modes: also computes)
   unsigned bar_target;         // whole-grid barrier
   unsigned ev0, ev1, ev2, ev3, ev4;   // split-phase barrier events completed so far (this launch), per chain
   unsigned round;              // rounds completed in this launch (parity of seed_raw / count buffers)
@@ -64,7 +64,6 @@ struct Ctx {
   long long* prof;             // profiling slots of this CTA in SHARED memory (null unless CTA 0 / G-1);
                                // flushed to global once, at kernel end, so timing does not stall the timed code
 #if FFN_PROFILE
-  long long* trace;            // per-tile event times of CTA kTraceCta (global, [kTraceEvents][kTraceTiles]); else null
   unsigned sig_cnt;            // signaller: releases so far
 #endif
   // mbarrier phase parities and pending-prefetch flags as ONE bit field: dynamically indexed arrays
@@ -90,6 +89,19 @@ __device__ __forceinline__ CanvasState* chain_state(const Ctx& c, int k) {
   return reinterpret_cast<CanvasState*>(reinterpret_cast<unsigned char*>(c.s_state) + k * kStateSlot);
 }
 
+// Tiles [tb, te) of chain k's conv stack on this CTA (the pipelined fp16 path).  Every chain cuts the nt tiles into
+// G contiguous ranges of nt / G or nt / G + 1 tiles, but the nt mod G longer ranges start at a different CTA for
+// every chain (CTA index rotated by k * (nt mod G)): a layer of a chain ends when its slowest CTA is done, and one
+// split shared by all chains would give the same CTAs the extra tile of every chain.  This way no CTA works through
+// more than ceil(K * nt / G) tiles of a K-chain round's layer.  Staging and pasting keep the per-CTA row split
+// [t_begin, t_end).
+__device__ __forceinline__ void chain_tiles(const Ctx& c, int k, int& tb, int& te) {
+  const int nt = c.p->g.nt, base = nt / c.G, extra = nt % c.G;
+  const int q = (c.cta + c.G - (k * extra) % c.G) % c.G;
+  tb = q * base + min(q, extra);
+  te = tb + base + (q < extra ? 1 : 0);
+}
+
 __device__ __forceinline__ bool aborted(const Ctx& c) {
   return sm90::ld_volatile_s32(c.p->ws.abort_flag) != 0;
 }
@@ -104,8 +116,11 @@ __device__ __forceinline__ void prof_add(const Ctx& c, int slot, long long dt) {
 // Tile timeline of one CTA (ffn_engine_trace): event e of the role's idx-th tile since kernel start.
 //   0 producer saw the chain barrier   1 tile's copies issued   2 consumers saw the operands   4 MMAs complete
 //   6 epilogue done   7 signaller released (idx = signal number)
+// The buffer ([kTraceEvents][kTraceTiles] after the counters) is looked up per event rather than kept in a
+// register: the fp16 path has none to spare.
 __device__ __forceinline__ void trace_ev(const Ctx& c, int ev, unsigned idx) {
-  if (c.trace && idx < (unsigned)kTraceTiles) c.trace[ev * kTraceTiles + idx] = clock64();
+  long long* trace = c.p->ws.prof;
+  if (trace && c.cta == kTraceCta && idx < (unsigned)kTraceTiles) trace[32 + ev * kTraceTiles + idx] = clock64();
 }
 #else
 __device__ __forceinline__ long long prof_now(const Ctx&) { return 0ll; }
@@ -375,11 +390,13 @@ __device__ __forceinline__ void tc_issue_weight_load(Ctx& c, int layer) {
 // and k-pair; the three dx taps ride along N.  `a_lo` / `b_lo` are the low descriptor words (start address,
 // LBO) of the warpgroup's first A row in the stage and of the layer's weights; every A start-address offset is
 // (const * seg_rows + const * xp).  Returns when the MMAs have completed (the stage may be released).
+// Straight-line code: the first MMA overwrites `d` (scale-d 0 is a compile-time constant, so `d` needs no
+// zero-fill) and ptxas keeps all of them in flight behind one wait.
 template <int NCH>
 __device__ __forceinline__ void tc_mma_tile(float (&d)[kAccRegs], uint32_t a_lo, uint32_t b_lo, int seg_rows, int xp) {
   const uint64_t hi = (uint64_t)(128u >> 4) << 32;   // SBO = 128 B
   sm90::wgmma_fence();
-#pragma unroll 1
+#pragma unroll
   for (int row = 0; row < 9; ++row) {
     const int tz = row / 3, ty = row % 3;
 #pragma unroll
@@ -438,7 +455,7 @@ __device__ __forceinline__ void tc_mma_tile_x2(float (&d)[kAccRegs], uint32_t aa
 enum EpiKind : int { EPI_A = 0, EPI_B_FIRST = 1, EPI_B = 2, EPI_LAST = 3 };
 
 template <int KIND, bool X2 = false>
-__device__ __forceinline__ int tc_epilogue(Ctx& c, int k, int layer, int j, const float (&d)[kAccRegs]) {
+__device__ __forceinline__ int tc_epilogue(Ctx& c, int k, int layer, int tile, const float (&d)[kAccRegs]) {
   const KParams& p = *c.p;
   const Geom& g = p.g;
   const ChainDev& ch = p.ch[k];
@@ -446,7 +463,6 @@ __device__ __forceinline__ int tc_epilogue(Ctx& c, int k, int layer, int j, cons
   constexpr bool kReadRes = KIND == EPI_B || KIND == EPI_LAST;
   constexpr bool kWriteRes = KIND == EPI_B_FIRST || KIND == EPI_B;
   const int t = c.lane & 3, gq = c.lane >> 2;
-  const int tile = c.t_begin + j;
   const int m0 = c.warp * 16 + gq;                     // accumulator rows of this thread: m0, m0 + 8
   float* xch = c.s_xchg + (c.epi_cnt & 1) * (8 * 2 * 4 * 8);   // double-buffered by tile parity
   // fragment index of (dx block b, row half h, channel slot q = 2 i + e): 4 * (4 b + i) + 2 h + e
@@ -544,7 +560,7 @@ __device__ __forceinline__ int tc_epilogue(Ctx& c, int k, int layer, int j, cons
       part += __shfl_xor_sync(0xffffffffu, part, 2);
       if (t == 0 && valid) {
         const float upd = part + c.s_bias[g.nconv * 32 + 32];
-        const float raw = raw_in[r];
+        const float raw = __ldcg(raw_in + r);   // staged by the CTA whose rows these are (chain_tiles), not this one
         const float fed = isnan(raw) ? p.cv.opt.pad_value : raw;
         const float logit = fed + upd;
         ch.logits[r] = logit;
@@ -558,11 +574,11 @@ __device__ __forceinline__ int tc_epilogue(Ctx& c, int k, int layer, int j, cons
 }
 
 template <bool X2>
-__device__ __forceinline__ int tc_epilogue_any(Ctx& c, int k, int layer, int j, const float (&d)[kAccRegs]) {
-  if (layer == c.p->g.nconv - 1) return tc_epilogue<EPI_LAST, X2>(c, k, layer, j, d);
-  if (!(layer & 1)) return tc_epilogue<EPI_A, X2>(c, k, layer, j, d);
-  if (layer == 1) return tc_epilogue<EPI_B_FIRST, X2>(c, k, layer, j, d);
-  return tc_epilogue<EPI_B, X2>(c, k, layer, j, d);
+__device__ __forceinline__ int tc_epilogue_any(Ctx& c, int k, int layer, int tile, const float (&d)[kAccRegs]) {
+  if (layer == c.p->g.nconv - 1) return tc_epilogue<EPI_LAST, X2>(c, k, layer, tile, d);
+  if (!(layer & 1)) return tc_epilogue<EPI_A, X2>(c, k, layer, tile, d);
+  if (layer == 1) return tc_epilogue<EPI_B_FIRST, X2>(c, k, layer, tile, d);
+  return tc_epilogue<EPI_B, X2>(c, k, layer, tile, d);
 }
 
 // Adds the per-row counts of the last layer (this warp's `hit`) to the chain's step counters.
@@ -597,9 +613,8 @@ __device__ __forceinline__ void layers_pipelined(Ctx& c, unsigned mask) {
   unsigned char* act_smem = c.smem + 2 * 27 * 4 * 512;
   const int seg_rows = kTileOut + 2 * g.halo;                 // k-chunk plane pitch of a stage (rows)
   const int stage_bytes = 3 * 4 * seg_rows * 16;
-  const int ntiles = c.t_end - c.t_begin;
   const int nconv = g.nconv;
-  const long long t_layers = prof_now(c);
+  if (c.tid == 0) prof_add(c, 11, -prof_now(c));   // + the time at the end (kept in the slot, not in a register)
 
   // The producer runs with the WHOLE warp converged (c.warp is warp-uniform by construction, see the kernel
   // entry) and elects one lane only for the instructions with side effects: addresses then live in uniform
@@ -625,7 +640,9 @@ __device__ __forceinline__ void layers_pipelined(Ctx& c, unsigned mask) {
 #ifndef FFN_EXP_NO_READER_FENCE
         sm90::fence_proxy_async_global();
 #endif        // other CTAs' generic-proxy stores (ordered by the acquire) -> async proxy
-        for (int j = 0; j < ntiles; ++j) {
+        int tb, te;
+        chain_tiles(c, k, tb, te);
+        for (int tile = tb; tile < te; ++tile) {
           const int s = c.load_cnt % kActStages;
           mbar_wait(c, &c.mb_empty[s], ((c.load_cnt / kActStages) & 1u) ^ 1u);
           if (weights_pending && c.load_cnt - n0 == (unsigned)(kActStages - 1)) {
@@ -633,7 +650,7 @@ __device__ __forceinline__ void layers_pipelined(Ctx& c, unsigned mask) {
             if (sm90::elect_one()) tc_issue_weight_load(c, (layer + 1 == nconv) ? 0 : layer + 1);
             __syncwarp();
           }
-          const int r0 = (c.t_begin + j) * kTileOut;
+          const int r0 = tile * kTileOut;
           unsigned char* dst = act_smem + (size_t)s * stage_bytes;
           if (sm90::elect_one()) {
             sm90::mbar_expect_tx(&c.mb_full[s], (uint32_t)(3 * nch * seg_rows * 16));
@@ -685,7 +702,9 @@ __device__ __forceinline__ void layers_pipelined(Ctx& c, unsigned mask) {
       for (int k = 0; k < kMaxChains; ++k) {
         if (!((mask >> k) & 1u)) continue;
         int hit = 0;
-        for (int j = 0; j < ntiles; ++j) {
+        int tb, te;
+        chain_tiles(c, k, tb, te);
+        for (int tile = tb; tile < te; ++tile) {
           const int s = c.epi_cnt % kActStages;
           t0 = prof_now(c);
           mbar_wait(c, &c.mb_full[s], (c.epi_cnt / kActStages) & 1u);
@@ -694,9 +713,7 @@ __device__ __forceinline__ void layers_pipelined(Ctx& c, unsigned mask) {
           t0 = prof_now(c);
           const uint32_t a_lo = (((sm90::smem_u32(act_smem + (size_t)s * stage_bytes) >> 4) & 0x3FFFu) + wg_rows) |
                                 ((uint32_t)(3 * seg_rows) << 16);
-          float d[kAccRegs];
-#pragma unroll
-          for (int i = 0; i < kAccRegs; ++i) d[i] = 0.f;
+          float d[kAccRegs];   // written by the tile's first MMA
           if (layer == 0) {
             tc_mma_tile<2>(d, a_lo, b_lo, seg_rows, g.xp);
           } else {
@@ -707,7 +724,7 @@ __device__ __forceinline__ void layers_pipelined(Ctx& c, unsigned mask) {
           if (c.tid == 0) prof_add(c, 3, prof_now(c) - t0);
           if (c.tid == 0) trace_ev(c, 4, c.epi_cnt);
           t0 = prof_now(c);
-          hit += tc_epilogue_any<false>(c, k, layer, j, d);
+          hit += tc_epilogue_any<false>(c, k, layer, tile, d);
           if (c.tid == 0) prof_add(c, 5, prof_now(c) - t0);
           if (c.tid == 0) trace_ev(c, 6, c.epi_cnt - 1u);
         }
@@ -725,7 +742,7 @@ __device__ __forceinline__ void layers_pipelined(Ctx& c, unsigned mask) {
 #pragma unroll
   for (int k = 0; k < kMaxChains; ++k)
     if ((mask >> k) & 1u) ev_add(c, k, (unsigned)nconv);   // staged + layers 0 .. nconv-2
-  if (c.tid == 0) prof_add(c, 11, prof_now(c) - t_layers);
+  if (c.tid == 0) prof_add(c, 11, prof_now(c));
 }
 
 // Near-fp32 tensor-core layer (FFN_COMPUTE_FP16X2_TC): activations and weights are both split into fp16
@@ -794,7 +811,7 @@ __device__ __forceinline__ void tc_layer_x2(Ctx& c, int layer) {
       tc_mma_tile_x2(d, aa_hi, aa_lo, bw_hi, bw_lo, nch, seg_rows, g.xp);
       __syncwarp();
       if (c.lane == 0) sm90::mbar_arrive(&c.mb_empty[0]);
-      hit += tc_epilogue_any<true>(c, 0, layer, j, d);
+      hit += tc_epilogue_any<true>(c, 0, layer, c.t_begin + j, d);
     }
     if (last) publish_counts(c, 0, hit);
   }
@@ -868,11 +885,12 @@ __device__ __forceinline__ void f32_layer(Ctx& c, int layer) {
 
 // Parity modes (fp32 FMA / split fp16): the conv stack of chain 0 with a whole-grid barrier after every
 // layer.  On return the caller's end-of-round grid barrier makes logits and counts visible.
+template <bool kSplit>
 __device__ __forceinline__ void layers_blocking(Ctx& c) {
   const KParams& p = *c.p;
   grid_barrier(c);   // staged operands visible
   for (int layer = 0; layer < p.g.nconv; ++layer) {
-    if (p.compute_mode == FFN_COMPUTE_FP16X2_TC) {
+    if constexpr (kSplit) {
       tc_layer_x2(c, layer);
     } else {
       f32_layer(c, layer);
@@ -2235,9 +2253,10 @@ __device__ __forceinline__ void commit_write(Ctx& c, int b) {   // inference.py:
 // The kernel
 // ------------------------------------------------------------------------------------------
 // One round = one FoV step of every chain in `mask` (staged by the caller with the current parity).
+template <bool kSplit>
 __device__ __forceinline__ void run_layers(Ctx& c, unsigned mask) {
   const KParams& p = *c.p;
-  if (p.compute_mode == FFN_COMPUTE_FP16_TC) {
+  if (!kSplit && p.compute_mode == FFN_COMPUTE_FP16_TC) {
     // the staged operands: every thread's stores, then one arrival per chain (event 1 of the round)
     __syncthreads();
     if (c.tid == 0) {
@@ -2247,10 +2266,14 @@ __device__ __forceinline__ void run_layers(Ctx& c, unsigned mask) {
     }
     layers_pipelined(c, mask);
   } else {
-    layers_blocking(c);
+    layers_blocking<kSplit>(c);
   }
 }
 
+// kSplit = true: the instance for FFN_COMPUTE_FP16X2_TC, false: FFN_COMPUTE_FP16_TC and FFN_COMPUTE_FP32.  ptxas
+// decides wgmma pipelining for a whole function, and the split-fp16 MMAs (tc_mma_tile_x2) in the same function as
+// the fp16 path make it wait for every fp16 MMA before issuing the next one.
+template <bool kSplit>
 __global__ void __launch_bounds__(kThreads, 1) ffn_flood_kernel(const __grid_constant__ KParams p) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   Ctx c;
@@ -2287,13 +2310,11 @@ __global__ void __launch_bounds__(kThreads, 1) ffn_flood_kernel(const __grid_con
   c.prof = nullptr;
   if (FFN_PROFILE && p.ws.prof && (c.cta == 0 || c.cta == c.G - 1)) {
     c.prof = reinterpret_cast<long long*>(smem_raw + L.bars + kOffProf);
-    if (c.tid < 16) c.prof[c.tid] = 0;
+    if (c.tid < 16) c.prof[c.tid] = c.tid == 10 ? -clock64() : 0;   // slot 10 (kernel time) adds the clock at exit
   }
 #if FFN_PROFILE
-  c.trace = (p.ws.prof && c.cta == kTraceCta) ? p.ws.prof + 32 : nullptr;
   c.sig_cnt = 0;
 #endif
-  const long long t_kernel = prof_now(c);
   c.bits = 0;
   const bool tc = p.compute_mode != FFN_COMPUTE_FP32;
   const int K = p.nchains;
@@ -2336,7 +2357,7 @@ __global__ void __launch_bounds__(kThreads, 1) ffn_flood_kernel(const __grid_con
           stage_fov(c, k, 0, 0, 0, 0, b0 + k);
           mask |= 1u << k;
         }
-      run_layers(c, mask);
+      run_layers<kSplit>(c, mask);
       grid_barrier(c);
       for (int k = 0; k < K; ++k)
         if ((mask >> k) & 1u) tail_paste(c, k, 0, c.round & 1u, 0, 0, 0, b0 + k, false);
@@ -2413,7 +2434,7 @@ __global__ void __launch_bounds__(kThreads, 1) ffn_flood_kernel(const __grid_con
       }
       if (c.tid == 0) prof_add(c, 6, prof_now(c) - t0);
       if (mask) {
-        run_layers(c, mask);
+        run_layers<kSplit>(c, mask);
         if (c.tid == 0) prof_add(c, 9, __popc(mask));
       }
       stepped = mask;
@@ -2421,7 +2442,7 @@ __global__ void __launch_bounds__(kThreads, 1) ffn_flood_kernel(const __grid_con
     }
   }
 
-  if (c.tid == 0) prof_add(c, 10, prof_now(c) - t_kernel);
+  if (c.tid == 0) prof_add(c, 10, prof_now(c));
   __syncthreads();
   if (c.prof && c.tid < 16) p.ws.prof[(c.cta == 0 ? 0 : 16) + c.tid] += c.prof[c.tid];
   // Teardown: no bulk copy may be in flight into this CTA's shared memory at exit (the fp16 path always
