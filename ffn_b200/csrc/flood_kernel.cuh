@@ -389,11 +389,12 @@ __device__ __forceinline__ void tc_issue_weight_load(Ctx& c, int layer) {
 // This warpgroup's 64 accumulator rows of one tile: 9 * NCH/2 MMAs 64 x 96 x 16, one per (dz, dy) tap-row
 // and k-pair; the three dx taps ride along N.  `a_lo` / `b_lo` are the low descriptor words (start address,
 // LBO) of the warpgroup's first A row in the stage and of the layer's weights; every A start-address offset is
-// (const * seg_rows + const * xp).  Returns when the MMAs have completed (the stage may be released).
+// (const * seg_rows + const * xp).  Returns with the MMAs in flight: `d` must not be touched, nor the stage
+// released, before sm90::wgmma_wait_all().
 // Straight-line code: the first MMA overwrites `d` (scale-d 0 is a compile-time constant, so `d` needs no
 // zero-fill) and ptxas keeps all of them in flight behind one wait.
 template <int NCH>
-__device__ __forceinline__ void tc_mma_tile(float (&d)[kAccRegs], uint32_t a_lo, uint32_t b_lo, int seg_rows, int xp) {
+__device__ __forceinline__ void tc_mma_issue(float (&d)[kAccRegs], uint32_t a_lo, uint32_t b_lo, int seg_rows, int xp) {
   const uint64_t hi = (uint64_t)(128u >> 4) << 32;   // SBO = 128 B
   sm90::wgmma_fence();
 #pragma unroll
@@ -407,7 +408,6 @@ __device__ __forceinline__ void tc_mma_tile(float (&d)[kAccRegs], uint32_t a_lo,
     }
   }
   sm90::wgmma_commit();
-  sm90::wgmma_wait_all();
 }
 
 // Split-fp16 form (FFN_COMPUTE_FP16X2_TC): stage layout [dz][k-chunk][row] for the hi parts at `aa_hi` and the lo
@@ -453,6 +453,25 @@ __device__ __forceinline__ void tc_mma_tile_x2(float (&d)[kAccRegs], uint32_t aa
 // lanes up / down with warp shuffles, plus a shared-memory exchange at the warp boundaries.  The fp32 residual
 // stream of every (chain, tile) lives in global memory (L2), in this thread order, read and written by the same thread.
 enum EpiKind : int { EPI_A = 0, EPI_B_FIRST = 1, EPI_B = 2, EPI_LAST = 3 };
+
+__device__ __forceinline__ int epi_kind(const Geom& g, int layer) {
+  if (layer == g.nconv - 1) return EPI_LAST;
+  if (!(layer & 1)) return EPI_A;
+  return layer == 1 ? EPI_B_FIRST : EPI_B;
+}
+
+// Brings the residual rows a tile's epilogue will read (EPI_B, EPI_LAST; the thread's rows m0 and m0 + 8) from L2 into
+// this SM's L1.  The fp16 path calls it just before a tile's MMAs, so that the L2 round trip overlaps the tensor-core
+// work and the epilogue's reads hit L1.  A prefetch rather than a load into registers: the fp16 kernel is at the 168
+// registers a 320-thread wgmma kernel can have (allocation covers three whole warpgroups), and 16 more live across
+// the MMAs make it spill.  The layer kind is tested at run time, so the code around the MMAs exists once.
+__device__ __forceinline__ void tc_prefetch_residual(const Ctx& c, int k, int layer, int tile) {
+  const int kind = epi_kind(c.p->g, layer);
+  if (kind != EPI_B && kind != EPI_LAST) return;
+  const float* res = c.p->ch[k].res + ((size_t)tile * kTileM + c.warp * 16 + (c.lane >> 2)) * kFeat + 8 * (c.lane & 3);
+  sm90::prefetch_l1(res);
+  sm90::prefetch_l1(res + 8 * kFeat);   // row m0 + 8
+}
 
 template <int KIND, bool X2 = false>
 __device__ __forceinline__ int tc_epilogue(Ctx& c, int k, int layer, int tile, const float (&d)[kAccRegs]) {
@@ -504,7 +523,6 @@ __device__ __forceinline__ int tc_epilogue(Ctx& c, int k, int layer, int tile, c
   }
   const size_t chunk_stride = (size_t)g.rows_alloc * 8;
   const float* bias = c.s_bias + layer * 32 + 2 * t;
-  const float* raw_in = ch.seed_raw[c.round & 1u];
   int hit = 0;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
@@ -517,8 +535,8 @@ __device__ __forceinline__ int tc_epilogue(Ctx& c, int k, int layer, int tile, c
     const float m_up = x == 0 ? 0.f : 1.f, m_dn = x == g.fx - 1 ? 0.f : 1.f;
     float* res = ch.res + ((size_t)tile * kTileM + m) * kFeat + 8 * t;
     float rr[8];
-    if (kReadRes) {
-      const float4 r0 = __ldcg(reinterpret_cast<const float4*>(res)), r1 = __ldcg(reinterpret_cast<const float4*>(res) + 1);
+    if (kReadRes) {   // through L1 (tc_prefetch_residual): only this CTA writes these lines, so L1 cannot be stale
+      const float4 r0 = __ldca(reinterpret_cast<const float4*>(res)), r1 = __ldca(reinterpret_cast<const float4*>(res) + 1);
       rr[0] = r0.x; rr[1] = r0.y; rr[2] = r0.z; rr[3] = r0.w; rr[4] = r1.x; rr[5] = r1.y; rr[6] = r1.z; rr[7] = r1.w;
     }
     float v[8];
@@ -560,7 +578,7 @@ __device__ __forceinline__ int tc_epilogue(Ctx& c, int k, int layer, int tile, c
       part += __shfl_xor_sync(0xffffffffu, part, 2);
       if (t == 0 && valid) {
         const float upd = part + c.s_bias[g.nconv * 32 + 32];
-        const float raw = __ldcg(raw_in + r);   // staged by the CTA whose rows these are (chain_tiles), not this one
+        const float raw = __ldcg(ch.seed_raw[c.round & 1u] + r);   // staged by the CTA whose rows these are (chain_tiles), not this one
         const float fed = isnan(raw) ? p.cv.opt.pad_value : raw;
         const float logit = fed + upd;
         ch.logits[r] = logit;
@@ -711,14 +729,16 @@ __device__ __forceinline__ void layers_pipelined(Ctx& c, unsigned mask) {
           if (c.tid == 0) prof_add(c, 1, prof_now(c) - t0);
           if (c.tid == 0) trace_ev(c, 2, c.epi_cnt);
           t0 = prof_now(c);
+          tc_prefetch_residual(c, k, layer, tile);   // lands in L1 while the MMAs run
           const uint32_t a_lo = (((sm90::smem_u32(act_smem + (size_t)s * stage_bytes) >> 4) & 0x3FFFu) + wg_rows) |
                                 ((uint32_t)(3 * seg_rows) << 16);
           float d[kAccRegs];   // written by the tile's first MMA
           if (layer == 0) {
-            tc_mma_tile<2>(d, a_lo, b_lo, seg_rows, g.xp);
+            tc_mma_issue<2>(d, a_lo, b_lo, seg_rows, g.xp);
           } else {
-            tc_mma_tile<4>(d, a_lo, b_lo, seg_rows, g.xp);
+            tc_mma_issue<4>(d, a_lo, b_lo, seg_rows, g.xp);
           }
+          sm90::wgmma_wait_all();
           __syncwarp();
           if (c.lane == 0) sm90::mbar_arrive(&c.mb_empty[s]);   // this warp's MMAs have read the stage
           if (c.tid == 0) prof_add(c, 3, prof_now(c) - t0);

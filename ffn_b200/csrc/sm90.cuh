@@ -68,6 +68,8 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const void* tmap, in
 __device__ __forceinline__ void tma_prefetch_desc(const void* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(tmap) : "memory");
 }
+// Brings the line holding `p` into this SM's L1 without occupying a register or waiting for it.
+__device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
 
 // ---------------------------------------------------------------- wgmma (warpgroup MMA)
 // Shared-memory matrix descriptor (cute::GMMA::GmmaDescriptor layout): start address [0,14), leading byte
