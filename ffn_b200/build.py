@@ -25,17 +25,15 @@ def up_to_date():
   return all(os.path.getmtime(d) <= t for d in DEPS)
 
 
-def build(force=False, verbose=False, defines=(), out=None):
-  """Builds the engine library.  `defines` / `out` produce an experiment variant next to it
-  (tools/build_variants.py); the product is always the default build."""
-  out = out or OUT
-  if out == OUT and not force and up_to_date():
+def build(force=False, verbose=False):
+  """Builds the engine library."""
+  if not force and up_to_date():
     return OUT
-  tmp = out + '.tmp%d' % os.getpid()   # linked next to the target and renamed over it: a reader never sees a partial file
+  tmp = OUT + '.tmp%d' % os.getpid()   # linked next to the target and renamed over it: a reader never sees a partial file
   cmd = [
       nvcc_path(), '-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '--default-stream', 'per-thread',
       '-Xcompiler', '-fPIC', '-shared', '-o', tmp, SRC, '-lcudart',
-  ] + ['-D%s' % d for d in defines]
+  ]
   if verbose:
     cmd.insert(1, '-Xptxas')
     cmd.insert(2, '-v')
@@ -44,10 +42,10 @@ def build(force=False, verbose=False, defines=(), out=None):
     if os.path.exists(tmp):
       os.unlink(tmp)
     raise RuntimeError('nvcc failed:\n%s\n%s' % (res.stdout, res.stderr))
-  os.replace(tmp, out)
+  os.replace(tmp, OUT)
   if verbose:
     sys.stderr.write(res.stderr)
-  return out
+  return OUT
 
 
 if __name__ == '__main__':

@@ -14,10 +14,7 @@ constexpr int kThreads = 320;     // warps 0-7: two consumer warpgroups (wgmma +
                                   // warp 9: signals the chains' split-phase barriers (the release stays off the epilogue's path)
 constexpr int kLoadWarp = 8;
 constexpr int kSigWarp = 9;
-#ifndef FFN_ACT_STAGES
-#define FFN_ACT_STAGES 3
-#endif
-constexpr int kActStages = FFN_ACT_STAGES;     // shared-memory ring of per-tile activation operands
+constexpr int kActStages = 3;     // shared-memory ring of per-tile activation operands
 constexpr int kTileM = 128;       // accumulator rows per tensor-core tile (two m64 warpgroup MMAs)
 constexpr int kTileOut = 126;     // FoV rows a tile OUTPUTS: the dx = -1/+1 partial sums live one row up/down, so
                                   // the first and last accumulator row of every tile only feed their neighbours
@@ -25,14 +22,8 @@ constexpr int kStackN = 96;       // MMA N: the three dx taps of a (dz, dy) tap-
 constexpr int kFeat = 32;         // feature maps of every hidden layer
 constexpr int kAccRegs = 64 * kStackN / 128;   // fp32 accumulators per consumer thread (m64n96 fragment)
 constexpr int kMaxConv = 32;      // 2 * depth limit
-#ifndef FFN_MAX_CHAINS
-#define FFN_MAX_CHAINS 4
-#endif
-#ifndef FFN_BUFS_PER_CHAIN
-#define FFN_BUFS_PER_CHAIN 6
-#endif
-constexpr int kMaxChains = FFN_MAX_CHAINS;     // flood-fill chains (execution slots) time-multiplexed over the SMs of one kernel
-constexpr int kBufsPerChain = FFN_BUFS_PER_CHAIN;  // object buffers per chain: finished objects that wait for their turn to commit are parked
+constexpr int kMaxChains = 4;     // flood-fill chains (execution slots) time-multiplexed over the SMs of one kernel
+constexpr int kBufsPerChain = 6;  // object buffers per chain: finished objects that wait for their turn to commit are parked
 constexpr int kMaxBufs = kMaxChains * kBufsPerChain;
 constexpr int kSplitShift = 10;   // FFN_COMPUTE_FP16X2_TC: weights are split as w * 2^10 = hi + lo (keeps lo a normal fp16
                                   // number for |w| down to ~1e-4); the epilogue scales the accumulators back (exact)
@@ -163,7 +154,6 @@ struct CanvasState {
   int seg_all;                // 1: segment_all mode, 0: segment_at mode
   int weak;                   // last object ended by 'seed_got_too_weak'
   int popped, pop_run, pop_pos[3];   // leader scratch: queue already popped for this round (phase A)
-  int start_max_id;           // Sched::max_id when the object started (scheduler experiments)
   int n_unstepped;            // segment_all: positions that passed Canvas.is_valid_pos but were not stepped on (the pop that ended the
                               // object as 'seed_got_too_weak', pops skipped by the restrictor): logged at the END of the trajectory
                               // buffer, because their verdict — and with it the reference's counters — depends on the labels too
@@ -252,7 +242,6 @@ struct Job {
   unsigned char* seed_status;   // [n_seeds] 0: not started, 1: taken by a chain
   long long round_cap;          // segment_all: rounds one launch may run (watchdog)
   long long watchdog_ns;        // wall-clock limit of one launch
-  int debug;                    // scheduler experiments (FFN_B200_DEBUG): 1 = treat every early run as conflicting, 2 = no early runs
 };
 
 struct KParams {
@@ -274,7 +263,6 @@ struct KParams {
   float* snap;            // snapshot seed array (see Sched::last_chain); null with one chain
   Job job;
   int compute_mode;
-  int act_smem_bytes;   // 3 * 4 * seg_rows_max * 16
 };
 
 // The small-structures area at SmemLayout::bars (byte offsets from there):

@@ -1,7 +1,6 @@
 // engine.cu — host side of libffn_b200.so: device context, weight packing, canvases, launches,
 // and the extern "C" entry points declared in include/ffn_b200.h.
 #include <algorithm>
-#include <chrono>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -842,16 +841,11 @@ int ffn_canvas_segment_all(FfnCanvas* c, const int32_t* seeds, int64_t n_seeds, 
   // trace (Canvas.history) run one object at a time.
   int K = 1;
   if (e->compute_mode == FFN_COMPUTE_FP16_TC && !c->cv.trace) K = chain_limit(e);
-  const auto t_enter = std::chrono::steady_clock::now();
-  auto since = [&](std::chrono::steady_clock::time_point t) {
-    return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count();
-  };
   if (ensure_bufs(c, K > 1 ? kBufsPerChain * K : 1)) {
     // not enough device memory for the object buffers of several chains: run one object at a time
     cudaGetLastError();
     K = 1;
   }
-  const double ms_bufs = since(t_enter);
   int* d_seeds = nullptr;
   FfnOrigin* d_orig = nullptr;
   FfnOverlap* d_ovl = nullptr;
@@ -933,12 +927,10 @@ int ffn_canvas_segment_all(FfnCanvas* c, const int32_t* seeds, int64_t n_seeds, 
   job.ovl_touched = d_touched;
   job.ovl_ids = ovl_ids;
   job.seed_status = d_status;
-  if (const char* dbg = std::getenv("FFN_B200_DEBUG")) job.debug = std::atoi(dbg);
   double secs = 0;
   long long launches = 0;
   int stuck = 0;
   int rc = 0;
-  const double ms_setup = since(t_enter);
   for (;;) {
     const long long before_steps = sc.steps_executed, before_idx = sc.commit_idx;
     const unsigned before_round = sc.round;
@@ -955,17 +947,6 @@ int ffn_canvas_segment_all(FfnCanvas* c, const int32_t* seeds, int64_t n_seeds, 
       return fail("scheduler state copy failed");
     }
     if (sc.all_done) break;
-    if ((job.debug & 64) && sc.steps_executed < job.step_budget) {   // a launch ended early without being done: why?
-      std::vector<CanvasState> dbg(kMaxBufs);
-      cudaMemcpy(dbg.data(), c->d_state, sizeof(CanvasState) * kMaxBufs, cudaMemcpyDeviceToHost);
-      std::fprintf(stderr, "[ffn] launch %lld ended early: commit_idx %lld / %lld owner %d round %u active %d %d %d\n", launches,
-                   sc.commit_idx, (long long)n_seeds, sc.owner, sc.round, sc.active[0], sc.active[1], sc.active[2]);
-      for (int b = 0; b < K * kBufsPerChain; ++b)
-        if (sc.bkind[b] > 0)
-          std::fprintf(stderr, "   buf %d kind %d seed %lld bround %d | phase %d seed %lld spec %d iters %lld fin_round %d have_cur %d\n", b,
-                       sc.bkind[b], sc.bseed[b], sc.bround[b], dbg[b].phase, dbg[b].seed_index, dbg[b].spec, dbg[b].iters,
-                       dbg[b].fin_round, dbg[b].have_cur);
-    }
     if (sc.overflow & 16) stuck = 3;   // the device watchdog tripped
     (void)before_round;
     if (stuck < 3) stuck = (sc.steps_executed == before_steps && sc.commit_idx == before_idx) ? stuck + 1 : 0;
@@ -982,7 +963,6 @@ int ffn_canvas_segment_all(FfnCanvas* c, const int32_t* seeds, int64_t n_seeds, 
       break;
     }
   }
-  const double ms_loop = since(t_enter);
   if (!rc && pull_state(c)) rc = 1;
   // ---- Canvas.seed shows the last object segment_at ran on: bring it into the canvas's own array
   if (!rc && (sc.last_in_snap || sc.last_chain > 0)) {
@@ -1026,9 +1006,6 @@ int ffn_canvas_segment_all(FfnCanvas* c, const int32_t* seeds, int64_t n_seeds, 
                    cudaMemcpyDeviceToHost) != cudaSuccess)
       rc = fail("overlaps copy failed");
   cleanup();
-  if (job.debug & 128)
-    std::fprintf(stderr, "[ffn] segment_all host ms: buffers %.2f, setup %.2f, launches %.2f (kernel %.2f), tail %.2f\n", ms_bufs,
-                 ms_setup - ms_bufs, ms_loop - ms_setup, secs * 1e3, since(t_enter) - ms_loop);
   st.ctr = sc.ctr;
   st.ctr.max_id = sc.max_id;
   st.ctr.device_seconds += secs;
@@ -1598,10 +1575,10 @@ int ffn_decision_points(int device, const FfnDecisionPointDesc* desc, uint64_t* 
   return 0;
 }
 
-int ffn_selftest_umma(int device, int variant, double* out, int n_out) {
+int ffn_selftest_wgmma(int device, double* out, int n_out) {
   if (!out || n_out < 8) return fail("need >= 8 output slots");
   std::string err;
-  if (ffn::selftest::run(device, variant, out, n_out, &err)) return fail(err);
+  if (ffn::selftest::run(device, out, n_out, &err)) return fail(err);
   return 0;
 }
 

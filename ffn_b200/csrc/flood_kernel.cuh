@@ -655,9 +655,7 @@ __device__ __forceinline__ void layers_pipelined(Ctx& c, unsigned mask) {
         const __half* in = layer == 0 ? ch.act0_h : ch.act_h[(layer - 1) & 1];
         chain_wait(c, k, (unsigned)layer + 1u);   // event 1 = staged, event l + 1 = layer l - 1 complete everywhere
         if (c.lane == 0) trace_ev(c, 0, c.load_cnt);
-#ifndef FFN_EXP_NO_READER_FENCE
-        sm90::fence_proxy_async_global();
-#endif        // other CTAs' generic-proxy stores (ordered by the acquire) -> async proxy
+        sm90::fence_proxy_async_global();   // other CTAs' generic-proxy stores (ordered by the acquire) -> async proxy
         int tb, te;
         chain_tiles(c, k, tb, te);
         for (int tile = tb; tile < te; ++tile) {
@@ -985,7 +983,7 @@ __device__ __forceinline__ float seed_value(const KParams& p, const LChain& L, i
   return __ldcg(p.ob[L.b].seed + cv_index(p.cv, z, y, x));
 }
 
-// Optional event log for debugging / history export (one chain only; lane 0 of the leader warp).
+// Optional event log for debugging / history export (one chain only; written by the leader warp).
 enum TraceEvent : int { EV_PUSH = 1, EV_POP_VALID = 2, EV_POP_INVALID = 3, EV_POP_THRESHOLD = 4, EV_POP_DONE = 5,
                         EV_STEP = 6, EV_SEED_INVALID = 7, EV_SEED_START = 8, EV_DELETED = 9 };
 __device__ __forceinline__ void trace_event(const KParams& p, CanvasState* st, int type, int z, int y, int x) {
@@ -1160,46 +1158,6 @@ __device__ __forceinline__ void policy_finish(const Ctx& c, const LChain& L) {
   __syncwarp();
 }
 
-// FaceMaxMovementPolicy.__next__ (movement.py:186-198) + Canvas.is_valid_pos (inference.py:312-346)
-// for queue entries; lane 0 only (used while the event trace records: per-candidate events in order).
-__device__ __forceinline__ bool pop_next(const KParams& p, const LChain& L, int& z, int& y, int& x) {
-  const Geom& g = p.g;
-  const ObjDev& ob = p.ob[L.b];
-  CanvasState* st = L.st;
-  while (st->q_head < st->q_tail) {
-    const int h = st->q_head++;
-    z = __ldcg(ob.q_pos + 3 * h);
-    y = __ldcg(ob.q_pos + 3 * h + 1);
-    x = __ldcg(ob.q_pos + 3 * h + 2);
-    const unsigned stamp = __ldcg(ob.lattice + lattice_index(p, st, z, y, x));
-    const bool inside = z >= 0 && y >= 0 && x >= 0 && z < p.cv.sz && y < p.cv.sy && x < p.cv.sx;
-    float v = 0.f;
-    int sg = 0;
-    if (inside) {
-      sg = __ldcg(p.cv.seg + cv_index(p.cv, z, y, x));
-      v = seed_value(p, L, z, y, x);
-    }
-    if (stamp == st->epoch) {
-      trace_event(p, st, EV_POP_DONE, z, y, x);
-      continue;
-    }
-    if (inside && v < p.cv.opt.move_threshold) {
-      st->ctr.skip_threshold++;
-      trace_event(p, st, EV_POP_THRESHOLD, z, y, x);
-      continue;
-    }
-    if (z - g.mz < 0 || y - g.my < 0 || x - g.mx < 0 || z + g.mz >= p.cv.sz || y + g.my >= p.cv.sy ||
-        x + g.mx >= p.cv.sx || sg > 0) {
-      st->ctr.skip_invalid_pos++;
-      trace_event(p, st, EV_POP_INVALID, z, y, x);
-      continue;
-    }
-    trace_event(p, st, EV_POP_VALID, z, y, x);
-    return true;
-  }
-  return false;
-}
-
 // quantize_probability(expit(v)) (storage.py:137-143, inference.py:655-657).
 __device__ __forceinline__ uint8_t quantize_prob(float logit) {
   const float pf = 1.0f / (1.0f + expf(-logit));
@@ -1219,12 +1177,12 @@ __device__ __forceinline__ uint8_t quantize_prob(float logit) {
 // rejected candidates costs two L2 round trips instead of two per candidate.  Exactly equivalent to the
 // sequential loop: a candidate's verdict depends only on state that pops do not modify (the done
 // lattice, the seed / label canvases, the masks), and the counters of the rejected candidates in
-// front of the first accepted one are added up from the ballot masks.
+// front of the first accepted one are added up from the ballot masks.  With the event trace on, every candidate
+// the sequential loop would examine gets its pop event, in queue order.
 // Returns true (all lanes) with the next position in z / y / x.
 __device__ __forceinline__ bool warp_pop(const KParams& p, const LChain& L, int lane, int& z, int& y, int& x) {
   const Geom& g = p.g;
   const CanvasDev& cv = p.cv;
-  const ChainDev& ch = p.ch[L.k];
   const ObjDev& ob = p.ob[L.b];
   CanvasState* st = L.st;
   // inference.py:503-505: value of the object's start voxel — the same for every candidate of this call
@@ -1243,25 +1201,14 @@ __device__ __forceinline__ bool warp_pop(const KParams& p, const LChain& L, int 
       cx = __ldcg(ob.q_pos + 3 * h + 2);
       const unsigned stamp = __ldcg(ob.lattice + lattice_index(p, st, cz, cy, cx));
       const bool inside = cz >= 0 && cy >= 0 && cx >= 0 && cz < cv.sz && cy < cv.sy && cx < cv.sx;
-      float v = 0.f, old = 0.f;
+      float v = 0.f;
       int sg = 0;
-      bool in_fov = false;
       if (inside) {
         const size_t i = cv_index(cv, cz, cy, cx);
         sg = __ldcg(cv.seg + i);
         if (cv.mask) restricted = __ldg(cv.mask + i) != 0;
-        if (st->have_cur) {
-          const int fz = cz - (st->cur[0] - g.mz), fy = cy - (st->cur[1] - g.my), fx = cx - (st->cur[2] - g.mx);
-          in_fov = fz >= 0 && fz < g.fz && fy >= 0 && fy < g.fy && fx >= 0 && fx < g.fx;
-          if (in_fov) {
-            const int row = fz * g.pp + fy * g.xp + fx;
-            v = __ldcg(ch.logits + row);
-            old = __ldcg(ch.seed_raw[L.par] + row);
-          }
-        }
-        if (!in_fov) v = __ldcg(ob.seed + i);
+        v = seed_value(p, L, cz, cy, cx);
       }
-      if (in_fov && L.disco && old < 0.f && v > old) v = old;
       const bool border = cz - g.mz < 0 || cy - g.my < 0 || cx - g.mx < 0 || cz + g.mz >= cv.sz ||
                           cy + g.my >= cv.sy || cx + g.mx >= cv.sx;
       if (stamp == st->epoch) {
@@ -1282,6 +1229,20 @@ __device__ __forceinline__ bool warp_pop(const KParams& p, const LChain& L, int 
     const unsigned m_stop = __ballot_sync(full, act && cls == 3 && (weak || !restricted));
     const int f = m_stop ? __ffs(m_stop) - 1 : -1;
     const unsigned before = f >= 0 ? ((1u << f) - 1u) : m_act;
+    if (cv.trace) {
+      // the candidates the sequential loop examines: the active ones up to and including the first stop
+      const unsigned m_ev = f >= 0 ? (before | (1u << f)) : m_act;
+      const int slot = st->n_trace + __popc(m_ev & ((1u << lane) - 1u));
+      if (((m_ev >> lane) & 1u) && slot < cv.trace_cap) {
+        int* t = cv.trace + 4 * slot;
+        t[0] = EV_POP_DONE - cls;   // class 0 done .. 3 valid -> EV_POP_DONE .. EV_POP_VALID
+        t[1] = cz;
+        t[2] = cy;
+        t[3] = cx;
+      }
+      __syncwarp();   // every lane has read n_trace
+      if (lane == 0) st->n_trace += __popc(m_ev);
+    }
     if (st->seg_all) {
       // Candidates that passed Canvas.is_valid_pos without being stepped on — skipped by the restrictor
       // (inference.py:507-509), or the one in hand when the loop ends with 'seed_got_too_weak' (:503-505) — relied on
@@ -1325,28 +1286,6 @@ __device__ __forceinline__ bool warp_pop(const KParams& p, const LChain& L, int 
   }
 }
 
-// The serial reference of warp_pop (lane 0 only): used when the event trace is recording, which
-// needs the per-candidate events in order.
-__device__ __forceinline__ bool serial_pop(const KParams& p, const LChain& L, int& z, int& y, int& x) {
-  const CanvasDev& cv = p.cv;
-  CanvasState* st = L.st;
-  for (;;) {
-    if (!pop_next(p, L, z, y, x)) return false;
-    // inference.py:503-505
-    if (seed_value(p, L, st->start[0], st->start[1], st->start[2]) < cv.opt.move_threshold) {
-      st->ctr.seed_got_too_weak++;
-      st->weak = 1;
-      return false;
-    }
-    // inference.py:507-509
-    if (cv.mask && cv.mask[cv_index(cv, z, y, x)]) {
-      st->ctr.skip_restricted_pos++;
-      continue;
-    }
-    return true;
-  }
-}
-
 // Pops the chain's queue (warp-collective) and parks the outcome in the state: the decision is then the
 // same whether this round goes on or the launch pauses (step budget) and a later launch resumes.
 __device__ __forceinline__ void chain_pop(const Ctx& c, const LChain& L) {
@@ -1354,17 +1293,7 @@ __device__ __forceinline__ void chain_pop(const Ctx& c, const LChain& L) {
   CanvasState* st = L.st;
   const long long t_pop = prof_now(c);
   int z = 0, y = 0, x = 0;
-  bool run;
-  if (p.cv.trace) {
-    run = false;
-    if (c.lane == 0) run = serial_pop(p, L, z, y, x);
-    run = __shfl_sync(0xffffffffu, (int)run, 0) != 0;
-    z = __shfl_sync(0xffffffffu, z, 0);
-    y = __shfl_sync(0xffffffffu, y, 0);
-    x = __shfl_sync(0xffffffffu, x, 0);
-  } else {
-    run = warp_pop(p, L, c.lane, z, y, x);
-  }
+  const bool run = warp_pop(p, L, c.lane, z, y, x);
   if (c.lane == 0) {
     st->popped = 1;
     st->pop_run = run ? 1 : 0;
@@ -1473,7 +1402,6 @@ __device__ __forceinline__ bool run_conflicts(const Ctx& c, int b, const CanvasS
 
 __device__ __forceinline__ void start_object(CanvasState* st, const Sched* sc, long long idx, int spec, int sz, int sy, int sx) {
   st->seed_index = idx;
-  st->start_max_id = sc->max_id;
   st->spec = spec;
   st->start[0] = sz;
   st->start[1] = sy;
@@ -1539,7 +1467,7 @@ __device__ __forceinline__ void lookahead(const Ctx& c, const LChain& L, Sched* 
   const int k = L.k;
   CanvasState* st = L.st;
   const unsigned full = 0xffffffffu;
-  if (sc->owner == L.b || p.nchains == 1 || (p.job.debug & 2)) return;
+  if (sc->owner == L.b || p.nchains == 1) return;
   constexpr int kWindow = 256;
   const long long base = sc->commit_idx + 1;
   for (int w = 0; w < kWindow; w += 32) {
@@ -1566,9 +1494,8 @@ __device__ __forceinline__ void lookahead(const Ctx& c, const LChain& L, Sched* 
           const CanvasState* o = chain_state(c, q);
           if (q == k || o->phase == PH_FREE) continue;
           // (measured on the 250^3 bench canvas: half a FoV of clearance beats a whole one for 3, 4 and 5 chains — fewer
-          // chain-rounds spent waiting; scheduler experiments: FFN_B200_DEBUG bit 256 = a whole FoV, bit 512 = two)
-          const int ms = (p.job.debug & 256) ? 2 : ((p.job.debug & 512) ? 4 : 1);
-          const int ez = g.fz * ms / 2, ey = g.fy * ms / 2, ex = g.fx * ms / 2;
+          // chain-rounds spent waiting)
+          const int ez = g.fz / 2, ey = g.fy / 2, ex = g.fx / 2;
           const bool has_box = o->dirty_hi[0] > o->dirty_lo[0];
           const int lo0 = (has_box ? min(o->dirty_lo[0], o->start[0]) : o->start[0]) - ez,
                     hi0 = (has_box ? max(o->dirty_hi[0], o->start[0] + 1) : o->start[0] + 1) + ez;
@@ -1582,11 +1509,10 @@ __device__ __forceinline__ void lookahead(const Ctx& c, const LChain& L, Sched* 
         // the seed order writes its labels before this seed's turn, and a seed inside it is then rejected by the
         // in-order gating (inference.py:562-568) — its run would be thrown away.  The object's own seed array says
         // which voxels it will label (>= segment_threshold, inference.py:635; NaN compares false).
-        if (!(p.job.debug & 32))
-          for (int b = 0; ok && b < p.nchains * kBufsPerChain; ++b)
-            if ((sc->bkind[b] == 1 || sc->bkind[b] == 2) && sc->bseed[b] >= 0 && sc->bseed[b] < j &&
-                __ldcg(p.ob[b].seed + i) >= cv.opt.segment_threshold)
-              ok = false;
+        for (int b = 0; ok && b < p.nchains * kBufsPerChain; ++b)
+          if ((sc->bkind[b] == 1 || sc->bkind[b] == 2) && sc->bseed[b] >= 0 && sc->bseed[b] < j &&
+              __ldcg(p.ob[b].seed + i) >= cv.opt.segment_threshold)
+            ok = false;
       }
     }
     const unsigned m = __ballot_sync(full, ok);
@@ -1724,7 +1650,7 @@ __device__ __forceinline__ int chain_advance(const Ctx& c, LChain L, Sched* sc, 
         // in-turn object (what Canvas.seed shows after segment_all), move that box to the snapshot array instead
         // of just clearing it
         int act = ACT_CLEAR;
-        if (st->seg_all && st->spec && sc->last_chain == L.b && !sc->last_in_snap && p.snap && !(p.job.debug & 8)) {
+        if (st->seg_all && st->spec && sc->last_chain == L.b && !sc->last_in_snap && p.snap) {
           act = ACT_CLEAR_MOVE;
           if (c.lane == 0) {
             for (int q = 0; q < 3; ++q) {
@@ -1839,8 +1765,7 @@ __device__ __forceinline__ int chain_advance(const Ctx& c, LChain L, Sched* sc, 
       if (st->spec) {
         int sz, sy, sx;
         const int ok = gate_seed(c, sc, st->seed_index, true, sz, sy, sx);   // the reference's gating, now, in order
-        const bool conflict = ok && (run_conflicts(c, L.b, st) || (p.job.debug & 1) ||
-                                     ((p.job.debug & 4) && sc->max_id != st->start_max_id));
+        const bool conflict = ok && run_conflicts(c, L.b, st);
         if (!ok || conflict) {
           if (c.lane == 0) {
             sc->spec_discarded++;
@@ -1947,7 +1872,6 @@ __device__ __forceinline__ int chain_advance(const Ctx& c, LChain L, Sched* sc, 
             o.start_zyx[2] = st->start[2];
             o.iters = st->iters;
             o.walltime_sec = (double)(sm90::globaltimer_ns() - st->seg_t0) * 1e-9;
-            if (p.job.debug & 16) o.walltime_sec = L.k * 1e5 + st->start_max_id;   // experiments
             p.job.origins[sc->n_origins] = o;
           } else {
             sc->overflow |= 4;

@@ -1,7 +1,6 @@
-// selftest.cuh — known-answer tests and micro-benchmarks of the sm_90a building blocks.
-// Not part of the product path: they pin the wgmma descriptor conventions the conv kernel relies on
-// (K-major, no-swizzle core matrices; shifted start addresses = convolution taps) and measure the
-// grid-barrier latency and the bulk-copy time.
+// selftest.cuh — known-answer test of the sm_90a wgmma descriptors.
+// Not part of the product path: it pins the wgmma descriptor conventions the conv kernel relies on
+// (K-major, no-swizzle core matrices; shifted start addresses = convolution taps).
 #pragma once
 
 #include <cuda_fp16.h>
@@ -17,15 +16,7 @@
 namespace ffn {
 namespace selftest {
 
-// Bounded spin: a broken descriptor must not hang the GPU box.
-__device__ __forceinline__ void bounded_wait(uint64_t* bar, uint32_t parity) {
-  const long long t0 = clock64();
-  while (!sm90::mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > (1ll << 31)) return;
-  }
-}
-
-// ---- variant 0: D[128 x 96] = A[128 x K] * B[96 x K]^T with explicit descriptors ------------
+// ---- D[128 x 96] = A[128 x K] * B[96 x K]^T with explicit descriptors ------------
 // Two warpgroups, 64 rows each, like the conv kernel's consumers.  A in smem: [k-chunk][row] 16-byte
 // units (row pitch 16 B, chunk pitch a_lbo); start address shifted by `a_shift_rows` rows (a
 // convolution tap).  B: [k-chunk][12 n-groups][8][8].
@@ -56,53 +47,6 @@ __global__ void wgmma_kat_kernel(const __half* a_g, int a_rows_total, const __ha
     const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
     d_out[(size_t)row * 96 + col] = d[i];
   }
-}
-
-// ---- variant 2: grid-barrier latency --------------------------------------------------------
-__global__ void barrier_kernel(unsigned* bar, int iters, long long* cycles_out) {
-  unsigned target = 0;
-  const long long t0 = clock64();
-  for (int i = 0; i < iters; ++i) {
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      target += gridDim.x;
-      __threadfence();
-      atomicAdd(bar, 1u);
-      const long long tw = clock64();
-      while (sm90::ld_acquire_u32(bar) < target) {
-        if (clock64() - tw > (1ll << 31)) break;
-      }
-      __threadfence();
-    }
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) cycles_out[blockIdx.x] = clock64() - t0;
-}
-
-// ---- variant 3: bulk-copy (TMA 1-D) of one layer's activation segments per CTA -----------------
-__global__ void bulk_kernel(const unsigned char* src, int pieces, int piece_bytes, int iters, long long* cycles_out) {
-  extern __shared__ __align__(1024) unsigned char smem[];
-  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + 131072);
-  if (threadIdx.x == 0) {
-    sm90::mbar_init(bar, 1);
-    sm90::fence_mbar_init();
-  }
-  __syncthreads();
-  uint32_t parity = 0;
-  const long long t0 = clock64();
-  for (int it = 0; it < iters; ++it) {
-    if (threadIdx.x == 0) {
-      sm90::mbar_expect_tx(bar, (uint32_t)(pieces * piece_bytes));
-      for (int i = 0; i < pieces; ++i)
-        sm90::bulk_g2s(smem + (size_t)i * piece_bytes,
-                        src + ((size_t)blockIdx.x * pieces + i) * piece_bytes + (size_t)(it & 7) * 16, (uint32_t)piece_bytes,
-                        bar);
-    }
-    bounded_wait(bar, parity);
-    parity ^= 1;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) cycles_out[blockIdx.x] = clock64() - t0;
 }
 
 inline float host_half_round(float v) { return __half2float(__float2half_rn(v)); }
@@ -172,61 +116,10 @@ inline int run_kat(double* out, std::string* err) {
   return 0;
 }
 
-inline int run(int device, int variant, double* out, int n_out, std::string* err) {
+inline int run(int device, double* out, int n_out, std::string* err) {
   ST_CUDA(cudaSetDevice(device));
-  cudaDeviceProp prop{};
-  ST_CUDA(cudaGetDeviceProperties(&prop, device));
   for (int i = 0; i < n_out; ++i) out[i] = -1.0;
-  if (variant == 0) return run_kat(out, err);
-  if (variant == 2) {
-    const int grid = prop.multiProcessorCount, iters = 200;
-    unsigned* d_bar = nullptr;
-    long long* d_c = nullptr;
-    ST_CUDA(cudaMalloc(&d_bar, 4));
-    ST_CUDA(cudaMalloc(&d_c, sizeof(long long) * grid));
-    for (int rep = 0; rep < 2; ++rep) {
-      ST_CUDA(cudaMemset(d_bar, 0, 4));
-      int it = iters;
-      void* args[] = {&d_bar, &it, &d_c};
-      ST_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<const void*>(barrier_kernel), dim3(grid), dim3(256), args, 0,
-                                          nullptr));
-      ST_CUDA(cudaDeviceSynchronize());
-    }
-    std::vector<long long> c(grid);
-    ST_CUDA(cudaMemcpy(c.data(), d_c, sizeof(long long) * grid, cudaMemcpyDeviceToHost));
-    long long worst = 0;
-    for (long long v : c) worst = std::max(worst, v);
-    out[0] = (double)worst / iters;   // cycles per grid barrier
-    out[1] = grid;
-    cudaFree(d_bar);
-    cudaFree(d_c);
-    return 0;
-  }
-  if (variant == 3) {
-    const int grid = prop.multiProcessorCount, iters = 500, pieces = 12, piece = 5216;
-    unsigned char* d_src = nullptr;
-    long long* d_c = nullptr;
-    ST_CUDA(cudaMalloc(&d_src, (size_t)grid * pieces * piece + 4096));
-    ST_CUDA(cudaMemset(d_src, 1, (size_t)grid * pieces * piece + 4096));
-    ST_CUDA(cudaMalloc(&d_c, sizeof(long long) * grid));
-    ST_CUDA(cudaFuncSetAttribute(bulk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 131072 + 64));
-    for (int rep = 0; rep < 2; ++rep) {
-      bulk_kernel<<<grid, 128, 131072 + 64>>>(d_src, pieces, piece, iters, d_c);
-      ST_CUDA(cudaGetLastError());
-      ST_CUDA(cudaDeviceSynchronize());
-    }
-    std::vector<long long> c(grid);
-    ST_CUDA(cudaMemcpy(c.data(), d_c, sizeof(long long) * grid, cudaMemcpyDeviceToHost));
-    long long worst = 0;
-    for (long long v : c) worst = std::max(worst, v);
-    out[0] = (double)worst / iters;   // cycles per 12 x 5216 B fetch, all SMs concurrently
-    out[1] = (double)pieces * piece;
-    cudaFree(d_src);
-    cudaFree(d_c);
-    return 0;
-  }
-  *err = "unknown selftest variant";
-  return 1;
+  return run_kat(out, err);
 }
 
 }  // namespace selftest

@@ -346,8 +346,8 @@ class DeviceCanvas:
     _lib.check(self._lib.ffn_canvas_add_id_offset(self._h, int(offset)))
 
 
-def selftest(variant: int, device: int = 0, n_out: int = 8) -> list:
+def selftest(device: int = 0, n_out: int = 8) -> list:
   lib = _lib.load()
   out = (C.c_double * n_out)()
-  _lib.check(lib.ffn_selftest_umma(int(device), int(variant), out, n_out))
+  _lib.check(lib.ffn_selftest_wgmma(int(device), out, n_out))
   return [float(v) for v in out]

@@ -1,8 +1,8 @@
 """FoV movement: host-side mirror of the policy objects whose state lives on the device.
 
 The per-step evaluation (face arg-max, threshold, descending sort, queue push/pop, quantised
-done-set) runs inside the persistent kernel (ffn_b200/csrc/flood_kernel.cuh: policy_update,
-pop_next).  This module keeps the reference's public surface — ffn/inference/movement.py:
+done-set) runs inside the persistent kernel (ffn_b200/csrc/flood_kernel.cuh: policy_finish,
+warp_pop).  This module keeps the reference's public surface — ffn/inference/movement.py:
 `get_scored_move_offsets` (:42-100), `BaseMovementPolicy` (:103-163), `FaceMaxMovementPolicy`
 (:166-222), `get_policy_fn` (:225-244), `MovementRestrictor` (:247-336) — so callers,
 checkpoints and request protos keep working.  `get_scored_move_offsets` is provided as a host

@@ -284,9 +284,9 @@ typedef struct {
 int ffn_decision_points(int device, const FfnDecisionPointDesc* desc, uint64_t* labels, FfnDecisionPoint* out,
                         int64_t cap, int64_t* n_out);
 
-/* Self tests / micro-benchmarks of the sm_90a building blocks (results in out[]; see
+/* Known-answer test of the wgmma descriptors (worst absolute error of each case in out[]; see
  * ffn_b200/csrc/selftest.cuh).  Used by tests, not by the product path. */
-int ffn_selftest_umma(int device, int variant, double* out, int n_out);
+int ffn_selftest_wgmma(int device, double* out, int n_out);
 
 #ifdef __cplusplus
 }

@@ -56,10 +56,10 @@ def _image(vol):
   return (vol.astype(np.float32) - np.float32(128.0)) / np.float32(33.0)
 
 
-def test_umma_descriptor_known_answer():
+def test_wgmma_descriptor_known_answer():
   """wgmma with the K-major / no-swizzle descriptors the conv kernel uses, incl. tap shifts."""
   from ffn_b200 import engine as eng
-  out = eng.selftest(0, n_out=16)
+  out = eng.selftest(n_out=16)
   assert out[0] == 0.0 and out[1] == 0.0 and out[2] == 0.0, out   # exact: small-integer operands
   assert out[3] > 1.0, 'swapped LBO/SBO must NOT reproduce the product'
 
