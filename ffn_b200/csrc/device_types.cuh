@@ -66,7 +66,13 @@ struct Weights {
 // Buffers shared by all chains (the fp32 / split-fp16 parity modes run one chain at a time).
 constexpr int kTraceEvents = 8, kTraceTiles = 2048, kTraceCta = 1;
 
+// Row geometry of the tensor-core epilogue (Workspace::row_flags), per accumulator row m of a tile: the FoV row
+// r = tile * kTileOut - 1 + m is an output row of this tile inside the FoV, x == 0 (no dx = -1 neighbour), x == fx - 1
+// (no dx = +1 neighbour).  A consumer thread's byte holds its rows m0 (bits 0-3) and m0 + 8 (bits 4-7).
+constexpr unsigned kRowValid = 1, kRowX0 = 2, kRowXLast = 4;
+
 struct Workspace {
+  const uint8_t* row_flags;   // [nt][8 warps][8 row groups] kRow* flags of a consumer thread's two rows (row_flags_byte)
   __half* act0_l;      // fp16 lo parts (FFN_COMPUTE_FP16X2_TC): x = hi + lo with hi = fp16(x), lo = fp16(x - hi)
   __half* act_l[2];
   float4* act0_f;      // [1][rows_alloc]  (image, seed, 0, 0)
@@ -280,7 +286,7 @@ constexpr int kMiscAbort = 7, kMiscDisco = 8, kMiscScratch = 16;
 constexpr int kOffRound = kOffMisc + (kMiscScratch + 32 * kMaxChains) * 4;
 constexpr int kOffProf = kOffRound + 2 * kMaxChains * 8 * 4;
 constexpr int kOffXchg = (kOffProf + 16 * 8 + 15) / 16 * 16;
-constexpr int kXchgBytes = 2 * 8 * 2 * 4 * 8 * 4;   // s_xchg: [2 tile parities][8 warps][2 directions][4 lanes][8]
+constexpr int kXchgBytes = 2 * 8 * 2 * 4 * 8 * 4;   // s_xchg: [2 tile parities][8 warps][2 directions][4 channel pairs][4 lanes][2]
 constexpr int kBarsAreaBytes = kOffXchg + kXchgBytes;
 
 // Shared-memory carve-up (bytes from the 1024-aligned base).
@@ -302,6 +308,25 @@ __host__ __device__ inline SmemLayout smem_layout(const Geom& g) {
   s.bars = s.bias + (kMaxConv + 1) * 32 * 4 + 16;
   s.total = s.bars + kBarsAreaBytes;
   return s;
+}
+
+// kRow* flags of accumulator row m of `tile`.  Rows that are not output rows keep x = 1, as the float decode of the
+// epilogue did: their values are stored to the residual stream but never read into a valid row.
+inline unsigned row_flags_of(const Geom& g, int tile, int m) {
+  const int r = tile * kTileOut - 1 + m;
+  int x = 1;
+  bool valid = false;
+  if (m >= 1 && m <= kTileOut && r >= 0 && r < g.nr) {
+    const int rem = r % g.pp, y = rem / g.xp;
+    x = rem % g.xp;
+    valid = y < g.fy;
+  }
+  return (valid ? kRowValid : 0u) | (x == 0 ? kRowX0 : 0u) | (x == g.fx - 1 ? kRowXLast : 0u);
+}
+
+inline uint8_t row_flags_byte(const Geom& g, int tile, int warp, int gq) {
+  const int m0 = warp * 16 + gq;
+  return (uint8_t)(row_flags_of(g, tile, m0) | row_flags_of(g, tile, m0 + 8) << 4);
 }
 
 __host__ __device__ inline size_t w16_layer_offset_halfs(int layer) {

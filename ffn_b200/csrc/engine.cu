@@ -490,6 +490,16 @@ int ffn_engine_create(int device, const FfnModelDesc* model, const float* const*
   for (void* p : std::vector<void*>{ws.act0_l, ws.act_l[0], ws.act_l[1], ws.act0_f, ws.act_f[0], ws.act_f[1], ws.res,
                                     ws.bar, ws.abort_flag, ws.prof})
     e->owned.push_back(p);
+  {
+    std::vector<uint8_t> flags((size_t)g.nt * 64);
+    for (int t = 0; t < g.nt; ++t)
+      for (int i = 0; i < 64; ++i) flags[(size_t)t * 64 + i] = row_flags_byte(g, t, i / 8, i % 8);
+    uint8_t* d_flags = nullptr;
+    if (dev_alloc(&d_flags, flags.size())) return 1;
+    e->owned.push_back(d_flags);
+    CUDA_OK(cudaMemcpy(d_flags, flags.data(), flags.size(), cudaMemcpyHostToDevice));
+    ws.row_flags = d_flags;
+  }
   for (int k = 0; k < kMaxChains; ++k) {   // per-chain step workspace: fp16 operands, raw seed, logits, counters, barrier,
     ChainDev& cw = e->cws[k];              // fp32 residual stream
     if (dev_alloc(&cw.act0_h, 2 * ra * 8)) return 1;

@@ -32,6 +32,8 @@
 
 #include <math_constants.h>
 
+#include <utility>
+
 #include "device_types.cuh"
 #include "sm90.cuh"
 
@@ -58,7 +60,7 @@ struct Ctx {
   unsigned load_cnt, epi_cnt;  // per-role running tile counters (ring index + phase parity)
   int* s_misc;                 // per-chain step-count accumulators, abort copy, disco flags, leader scratch (device_types.cuh: kOffMisc)
   int* s_round;                // [k][8] this round: action, z, y, x, buffer ; [kMaxChains + k][8] previous step: flags, z, y, x, buffer
-  float* s_xchg;               // [2 tile parities][8 warps][2 directions][4 lanes][8] partial sums crossing warp boundaries
+  float* s_xchg;               // [2 tile parities][8 warps][2 directions][4 channel pairs][4 lanes][2] partial sums crossing warp boundaries
   CanvasState* s_state;        // CTA 0: shared-memory working copies of the chain states (512-byte slots)
   Sched* s_sched;              // CTA 0: working copy of the scheduler state
   long long* prof;             // profiling slots of this CTA in SHARED memory (null unless CTA 0 / G-1);
@@ -393,20 +395,20 @@ __device__ __forceinline__ void tc_issue_weight_load(Ctx& c, int layer) {
 // released, before sm90::wgmma_wait_all().
 // Straight-line code: the first MMA overwrites `d` (scale-d 0 is a compile-time constant, so `d` needs no
 // zero-fill) and ptxas keeps all of them in flight behind one wait.
-template <int NCH>
-__device__ __forceinline__ void tc_mma_issue(float (&d)[kAccRegs], uint32_t a_lo, uint32_t b_lo, int seg_rows, int xp) {
-  const uint64_t hi = (uint64_t)(128u >> 4) << 32;   // SBO = 128 B
+// MMA I of the tile: tap-row I / (NCH / 2), k-pair I % (NCH / 2).  The weight offset is a template constant, so that
+// the descriptor is formed from `b_lo` at the MMA (sm90::wgmma_m64n96k16_lo).
+template <int NCH, int I>
+__device__ __forceinline__ void tc_mma_one(float (&d)[kAccRegs], uint32_t a_lo, uint32_t b_lo, int seg_rows, int xp) {
+  constexpr int row = I / (NCH / 2), j = I % (NCH / 2), tz = row / 3, ty = row % 3;
+  const uint32_t aoff = (uint32_t)((2 * j * 3 + tz) * seg_rows + ty * xp);   // stage layout [k-chunk][dz][row]
+  constexpr uint32_t boff = (uint32_t)((row * NCH + 2 * j) * (12 * 128 / 16));
+  sm90::wgmma_m64n96k16_lo<boff>(d, a_lo + aoff, b_lo, 128u >> 4 /* SBO = 128 B */, I != 0 ? 1u : 0u);
+}
+template <int NCH, int... I>
+__device__ __forceinline__ void tc_mma_issue(float (&d)[kAccRegs], uint32_t a_lo, uint32_t b_lo, int seg_rows, int xp,
+                                             std::integer_sequence<int, I...>) {
   sm90::wgmma_fence();
-#pragma unroll
-  for (int row = 0; row < 9; ++row) {
-    const int tz = row / 3, ty = row % 3;
-#pragma unroll
-    for (int j = 0; j < NCH / 2; ++j) {
-      const uint32_t aoff = (uint32_t)((2 * j * 3 + tz) * seg_rows + ty * xp);   // stage layout [k-chunk][dz][row]
-      const uint32_t boff = (uint32_t)((row * NCH + 2 * j) * (12 * 128 / 16));
-      sm90::wgmma_m64n96k16(d, hi | (uint64_t)(a_lo + aoff), hi | (uint64_t)(b_lo + boff), (row | j) != 0 ? 1u : 0u);
-    }
-  }
+  (tc_mma_one<NCH, I>(d, a_lo, b_lo, seg_rows, xp), ...);
   sm90::wgmma_commit();
 }
 
@@ -460,24 +462,43 @@ __device__ __forceinline__ int epi_kind(const Geom& g, int layer) {
   return layer == 1 ? EPI_B_FIRST : EPI_B;
 }
 
+// Where a consumer thread's epilogue writes for one (chain, layer), formed once where the chain is chosen: its residual
+// row m0 of tile 0, and its fp16 output of the FoV row that accumulator row m0 of tile 0 computes (k-chunk 0).  A tile
+// adds a 32-bit offset; row m0 + 8 and the other k-chunks are a constant or one stride away.
+struct EpiBase {
+  float* res;
+  __half* act;
+};
+__device__ __forceinline__ EpiBase epi_base(const Ctx& c, int k, int layer) {
+  const ChainDev& ch = c.p->ch[k];
+  const int t = c.lane & 3, m0 = c.warp * 16 + (c.lane >> 2);
+  return {ch.res + m0 * kFeat + 8 * t, ch.act_h[layer & 1] + (c.p->g.guard - 1 + m0) * 8 + 2 * t};
+}
+
+// This thread's byte of Workspace::row_flags for `tile`: the kRow* flags of its rows m0 (low half) and m0 + 8.
+__device__ __forceinline__ unsigned tc_row_flags(const Ctx& c, int tile) {
+  return __ldg(c.p->ws.row_flags + tile * 64 + c.warp * 8 + (c.lane >> 2));
+}
+
 // Brings the residual rows a tile's epilogue will read (EPI_B, EPI_LAST; the thread's rows m0 and m0 + 8) from L2 into
 // this SM's L1.  The fp16 path calls it just before a tile's MMAs, so that the L2 round trip overlaps the tensor-core
 // work and the epilogue's reads hit L1.  A prefetch rather than a load into registers: the fp16 kernel is at the 168
 // registers a 320-thread wgmma kernel can have (allocation covers three whole warpgroups), and 16 more live across
 // the MMAs make it spill.  The layer kind is tested at run time, so the code around the MMAs exists once.
-__device__ __forceinline__ void tc_prefetch_residual(const Ctx& c, int k, int layer, int tile) {
+__device__ __forceinline__ void tc_prefetch_residual(const Ctx& c, const EpiBase& e, int layer, int tile) {
   const int kind = epi_kind(c.p->g, layer);
   if (kind != EPI_B && kind != EPI_LAST) return;
-  const float* res = c.p->ch[k].res + ((size_t)tile * kTileM + c.warp * 16 + (c.lane >> 2)) * kFeat + 8 * (c.lane & 3);
+  const float* res = e.res + tile * (kTileM * kFeat);
   sm90::prefetch_l1(res);
   sm90::prefetch_l1(res + 8 * kFeat);   // row m0 + 8
 }
 
+// `flags`: tc_row_flags of the tile, loaded by the caller before the MMAs complete.
 template <int KIND, bool X2 = false>
-__device__ __forceinline__ int tc_epilogue(Ctx& c, int k, int layer, int tile, const float (&d)[kAccRegs]) {
+__device__ __forceinline__ int tc_epilogue(Ctx& c, int k, int layer, int tile, const EpiBase& e, unsigned flags,
+                                           const float (&d)[kAccRegs]) {
   const KParams& p = *c.p;
   const Geom& g = p.g;
-  const ChainDev& ch = p.ch[k];
   constexpr float kUnscale = 1.0f / (float)(1 << kSplitShift);   // X2: accumulators carry w * 2^kSplitShift
   constexpr bool kReadRes = KIND == EPI_B || KIND == EPI_LAST;
   constexpr bool kWriteRes = KIND == EPI_B_FIRST || KIND == EPI_B;
@@ -486,15 +507,16 @@ __device__ __forceinline__ int tc_epilogue(Ctx& c, int k, int layer, int tile, c
   float* xch = c.s_xchg + (c.epi_cnt & 1) * (8 * 2 * 4 * 8);   // double-buffered by tile parity
   // fragment index of (dx block b, row half h, channel slot q = 2 i + e): 4 * (4 b + i) + 2 h + e
 #define ACC(b, h, q) d[4 * (4 * (b) + ((q) >> 1)) + 2 * (h) + ((q) & 1)]
+  // [warp][direction][channel pair i][lane t] float2: a pair is two adjacent accumulator registers, and pairs of one lane
+  // are not adjacent in memory, so they are stored and loaded as they are (four channels of a float4 are not)
+  float2* const x2 = reinterpret_cast<float2*>(xch);
   if (gq == 7) {   // row 15 of the dx = -1 block: consumed by row 0 of the next warp
-    float4* q4 = reinterpret_cast<float4*>(xch + ((c.warp * 2 + 0) * 4 + t) * 8);
-    q4[0] = make_float4(ACC(0, 1, 0), ACC(0, 1, 1), ACC(0, 1, 2), ACC(0, 1, 3));
-    q4[1] = make_float4(ACC(0, 1, 4), ACC(0, 1, 5), ACC(0, 1, 6), ACC(0, 1, 7));
+#pragma unroll
+    for (int i = 0; i < 4; ++i) x2[((c.warp * 2 + 0) * 4 + i) * 4 + t] = make_float2(ACC(0, 1, 2 * i), ACC(0, 1, 2 * i + 1));
   }
   if (gq == 0) {   // row 0 of the dx = +1 block: consumed by row 15 of the previous warp
-    float4* q4 = reinterpret_cast<float4*>(xch + ((c.warp * 2 + 1) * 4 + t) * 8);
-    q4[0] = make_float4(ACC(2, 0, 0), ACC(2, 0, 1), ACC(2, 0, 2), ACC(2, 0, 3));
-    q4[1] = make_float4(ACC(2, 0, 4), ACC(2, 0, 5), ACC(2, 0, 6), ACC(2, 0, 7));
+#pragma unroll
+    for (int i = 0; i < 4; ++i) x2[((c.warp * 2 + 1) * 4 + i) * 4 + t] = make_float2(ACC(2, 0, 2 * i), ACC(2, 0, 2 * i + 1));
   }
   asm volatile("bar.sync 3, 256;" ::: "memory");
   // up[h][q] = D[m-1][dx=-1], dn[h][q] = D[m+1][dx=+1] for the rows m = m0 + 8 h
@@ -510,30 +532,36 @@ __device__ __forceinline__ int tc_epilogue(Ctx& c, int k, int layer, int tile, c
     dn[1][q] = yb;                    // row m0 + 9 (gq = 7: next warp, below)
   }
   if (gq == 0 && c.warp > 0) {
-    const float4* q4 = reinterpret_cast<const float4*>(xch + (((c.warp - 1) * 2 + 0) * 4 + t) * 8);
-    const float4 u0 = q4[0], u1 = q4[1];
-    up[0][0] = u0.x; up[0][1] = u0.y; up[0][2] = u0.z; up[0][3] = u0.w;
-    up[0][4] = u1.x; up[0][5] = u1.y; up[0][6] = u1.z; up[0][7] = u1.w;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const float2 u = x2[(((c.warp - 1) * 2 + 0) * 4 + i) * 4 + t];
+      up[0][2 * i] = u.x;
+      up[0][2 * i + 1] = u.y;
+    }
   }
   if (gq == 7 && c.warp < 7) {
-    const float4* q4 = reinterpret_cast<const float4*>(xch + (((c.warp + 1) * 2 + 1) * 4 + t) * 8);
-    const float4 u0 = q4[0], u1 = q4[1];
-    dn[1][0] = u0.x; dn[1][1] = u0.y; dn[1][2] = u0.z; dn[1][3] = u0.w;
-    dn[1][4] = u1.x; dn[1][5] = u1.y; dn[1][6] = u1.z; dn[1][7] = u1.w;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const float2 u = x2[(((c.warp + 1) * 2 + 1) * 4 + i) * 4 + t];
+      dn[1][2 * i] = u.x;
+      dn[1][2 * i + 1] = u.y;
+    }
   }
-  const size_t chunk_stride = (size_t)g.rows_alloc * 8;
+  const int chunk_stride = g.rows_alloc * 8;           // halfs between k-chunks of an activation buffer
+  float* const res0 = e.res + tile * (kTileM * kFeat);
+  __half* const act0 = e.act + tile * (kTileOut * 8);
   const float* bias = c.s_bias + layer * 32 + 2 * t;
   int hit = 0;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int m = m0 + 8 * h;
     const int r = tile * kTileOut - 1 + m;             // FoV row of accumulator row m
-    int z = 0, y = 0, x = 1;
-    const bool valid = m >= 1 && m <= kTileOut && r >= 0 && row_to_zyx(g, r, z, y, x);
+    const unsigned f = flags >> (4 * h);
+    const bool valid = (f & kRowValid) != 0;
     // SAME padding in x: at x = 0 / x = fx-1 row v-1 / v+1 belongs to the neighbouring line (mask 0);
     // all partial sums are finite (pad rows multiply zero activations), so 0 * value is exact
-    const float m_up = x == 0 ? 0.f : 1.f, m_dn = x == g.fx - 1 ? 0.f : 1.f;
-    float* res = ch.res + ((size_t)tile * kTileM + m) * kFeat + 8 * t;
+    const float m_up = (f & kRowX0) ? 0.f : 1.f, m_dn = (f & kRowXLast) ? 0.f : 1.f;
+    float* res = res0 + 8 * h * kFeat;
     float rr[8];
     if (kReadRes) {   // through L1 (tc_prefetch_residual): only this CTA writes these lines, so L1 cannot be stale
       const float4 r0 = __ldca(reinterpret_cast<const float4*>(res)), r1 = __ldca(reinterpret_cast<const float4*>(res) + 1);
@@ -556,16 +584,17 @@ __device__ __forceinline__ int tc_epilogue(Ctx& c, int k, int layer, int tile, c
       if (valid) {
         // out = relu(.) as fp16: the ReLU rides on the conversion (cvt.rn.relu.f16x2.f32); channels 8 i + 2 t, +1 are
         // one half2 of k-chunk i ([k-chunk][row][8 halfs])
-        __half* dst = ch.act_h[layer & 1] + ((size_t)g.guard + r) * 8 + 2 * t;
+        __half* dst = act0 + 8 * 8 * h;
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
           const uint32_t o = sm90::cvt_relu_f16x2(v[2 * i], v[2 * i + 1]);
-          *reinterpret_cast<uint32_t*>(dst + i * chunk_stride) = o;
+          *reinterpret_cast<uint32_t*>(dst) = o;
           if (X2) {   // lo parts of relu(v): relu(v) - fp16(relu(v)) is exact in fp32
             const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&o));
             const __half2 l = __floats2half2_rn(fmaxf(v[2 * i], 0.f) - hf.x, fmaxf(v[2 * i + 1], 0.f) - hf.y);
-            *reinterpret_cast<__half2*>(p.ws.act_l[layer & 1] + ((size_t)g.guard + r) * 8 + 2 * t + i * chunk_stride) = l;
+            *reinterpret_cast<__half2*>(p.ws.act_l[layer & 1] + ((size_t)g.guard + r) * 8 + 2 * t + (size_t)i * chunk_stride) = l;
           }
+          dst += chunk_stride;
         }
       }
     } else {
@@ -577,6 +606,7 @@ __device__ __forceinline__ int tc_epilogue(Ctx& c, int k, int layer, int tile, c
       part += __shfl_xor_sync(0xffffffffu, part, 1);
       part += __shfl_xor_sync(0xffffffffu, part, 2);
       if (t == 0 && valid) {
+        const ChainDev& ch = p.ch[k];
         const float upd = part + c.s_bias[g.nconv * 32 + 32];
         const float raw = __ldcg(ch.seed_raw[c.round & 1u] + r);   // staged by the CTA whose rows these are (chain_tiles), not this one
         const float fed = isnan(raw) ? p.cv.opt.pad_value : raw;
@@ -592,11 +622,12 @@ __device__ __forceinline__ int tc_epilogue(Ctx& c, int k, int layer, int tile, c
 }
 
 template <bool X2>
-__device__ __forceinline__ int tc_epilogue_any(Ctx& c, int k, int layer, int tile, const float (&d)[kAccRegs]) {
-  if (layer == c.p->g.nconv - 1) return tc_epilogue<EPI_LAST, X2>(c, k, layer, tile, d);
-  if (!(layer & 1)) return tc_epilogue<EPI_A, X2>(c, k, layer, tile, d);
-  if (layer == 1) return tc_epilogue<EPI_B_FIRST, X2>(c, k, layer, tile, d);
-  return tc_epilogue<EPI_B, X2>(c, k, layer, tile, d);
+__device__ __forceinline__ int tc_epilogue_any(Ctx& c, int k, int layer, int tile, const EpiBase& e, unsigned flags,
+                                               const float (&d)[kAccRegs]) {
+  if (layer == c.p->g.nconv - 1) return tc_epilogue<EPI_LAST, X2>(c, k, layer, tile, e, flags, d);
+  if (!(layer & 1)) return tc_epilogue<EPI_A, X2>(c, k, layer, tile, e, flags, d);
+  if (layer == 1) return tc_epilogue<EPI_B_FIRST, X2>(c, k, layer, tile, e, flags, d);
+  return tc_epilogue<EPI_B, X2>(c, k, layer, tile, e, flags, d);
 }
 
 // Adds the per-row counts of the last layer (this warp's `hit`) to the chain's step counters.
@@ -720,6 +751,7 @@ __device__ __forceinline__ void layers_pipelined(Ctx& c, unsigned mask) {
         int hit = 0;
         int tb, te;
         chain_tiles(c, k, tb, te);
+        const EpiBase e = epi_base(c, k, layer);
         for (int tile = tb; tile < te; ++tile) {
           const int s = c.epi_cnt % kActStages;
           t0 = prof_now(c);
@@ -727,22 +759,23 @@ __device__ __forceinline__ void layers_pipelined(Ctx& c, unsigned mask) {
           if (c.tid == 0) prof_add(c, 1, prof_now(c) - t0);
           if (c.tid == 0) trace_ev(c, 2, c.epi_cnt);
           t0 = prof_now(c);
-          tc_prefetch_residual(c, k, layer, tile);   // lands in L1 while the MMAs run
+          tc_prefetch_residual(c, e, layer, tile);   // lands in L1 while the MMAs run
           const uint32_t a_lo = (((sm90::smem_u32(act_smem + (size_t)s * stage_bytes) >> 4) & 0x3FFFu) + wg_rows) |
                                 ((uint32_t)(3 * seg_rows) << 16);
           float d[kAccRegs];   // written by the tile's first MMA
           if (layer == 0) {
-            tc_mma_issue<2>(d, a_lo, b_lo, seg_rows, g.xp);
+            tc_mma_issue<2>(d, a_lo, b_lo, seg_rows, g.xp, std::make_integer_sequence<int, 9>{});
           } else {
-            tc_mma_issue<4>(d, a_lo, b_lo, seg_rows, g.xp);
+            tc_mma_issue<4>(d, a_lo, b_lo, seg_rows, g.xp, std::make_integer_sequence<int, 18>{});
           }
+          const unsigned flags = tc_row_flags(c, tile);   // the load's latency runs under the MMAs
           sm90::wgmma_wait_all();
           __syncwarp();
           if (c.lane == 0) sm90::mbar_arrive(&c.mb_empty[s]);   // this warp's MMAs have read the stage
           if (c.tid == 0) prof_add(c, 3, prof_now(c) - t0);
           if (c.tid == 0) trace_ev(c, 4, c.epi_cnt);
           t0 = prof_now(c);
-          hit += tc_epilogue_any<false>(c, k, layer, tile, d);
+          hit += tc_epilogue_any<false>(c, k, layer, tile, e, flags, d);
           if (c.tid == 0) prof_add(c, 5, prof_now(c) - t0);
           if (c.tid == 0) trace_ev(c, 6, c.epi_cnt - 1u);
         }
@@ -821,6 +854,7 @@ __device__ __forceinline__ void tc_layer_x2(Ctx& c, int layer) {
     const uint32_t bw_lo = ((sm90::smem_u32(c.smem + 27 * 4 * 512) >> 4) & 0x3FFFu) | ((12u * 128u >> 4) << 16);
     const uint32_t aa_hi = (((sm90::smem_u32(act_smem) >> 4) & 0x3FFFu) + wg_rows) | ((uint32_t)seg_rows << 16);
     const uint32_t aa_lo = (((sm90::smem_u32(act_smem + stage_bytes) >> 4) & 0x3FFFu) + wg_rows) | ((uint32_t)seg_rows << 16);
+    const EpiBase e = epi_base(c, 0, layer);
     for (int j = 0; j < ntiles; ++j) {
       mbar_wait(c, &c.mb_full[0], c.epi_cnt & 1u);
       float d[kAccRegs];
@@ -829,7 +863,7 @@ __device__ __forceinline__ void tc_layer_x2(Ctx& c, int layer) {
       tc_mma_tile_x2(d, aa_hi, aa_lo, bw_hi, bw_lo, nch, seg_rows, g.xp);
       __syncwarp();
       if (c.lane == 0) sm90::mbar_arrive(&c.mb_empty[0]);
-      hit += tc_epilogue_any<true>(c, 0, layer, c.t_begin + j, d);
+      hit += tc_epilogue_any<true>(c, 0, layer, c.t_begin + j, e, tc_row_flags(c, c.t_begin + j), d);
     }
     if (last) publish_counts(c, 0, hit);
   }

@@ -107,6 +107,29 @@ __device__ __forceinline__ void wgmma_m64n96k16(float (&d)[48], uint64_t adesc, 
       : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
 
+// The same MMA with both descriptors given as low words (start address, LBO) plus one shared high word (SBO), and B's
+// low word as b_lo + kBOff.  The compiler cannot hoist an addition inside the asm out of a loop, so B's descriptor is
+// formed at the point of use from one base, instead of one register pair per MMA being held across the loop.
+template <uint32_t kBOff>
+__device__ __forceinline__ void wgmma_m64n96k16_lo(float (&d)[48], uint32_t a_lo, uint32_t b_lo, uint32_t hi,
+                                                   uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .b32 bl;\n\t.reg .b64 ad, bd;\n\t"
+      "setp.ne.b32 p, %51, 0;\n\t"
+      "add.u32 bl, %49, %52;\n\t"
+      "mov.b64 ad, {%48, %50};\n\t"
+      "mov.b64 bd, {bl, %50};\n\t"
+      "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, ad, bd, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+      : "r"(a_lo), "r"(b_lo), "r"(hi), "r"(accumulate), "n"(kBOff));
+}
+
 // ---------------------------------------------------------------- misc
 __device__ __forceinline__ uint32_t ld_acquire_u32(const uint32_t* p) {
   uint32_t v;
