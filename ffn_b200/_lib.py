@@ -34,7 +34,7 @@ EXPORTS = [
     'ffn_canvas_update_at', 'ffn_canvas_init_seed', 'ffn_canvas_read', 'ffn_canvas_write',
     'ffn_canvas_policy_state_size', 'ffn_canvas_policy_state_get', 'ffn_canvas_policy_state_set',
     'ffn_canvas_set_resume', 'ffn_canvas_trace', 'ffn_canvas_seed_peaks', 'ffn_canvas_seed_policy', 'ffn_canvas_set_max_id', 'ffn_canvas_get_counters', 'ffn_canvas_spec_stats', 'ffn_canvas_device_ptr',
-    'ffn_canvas_add_id_offset', 'ffn_decision_points', 'ffn_selftest_wgmma',
+    'ffn_canvas_add_id_offset', 'ffn_decision_points', 'ffn_reseg_eval', 'ffn_selftest_wgmma',
 ]
 
 
@@ -78,6 +78,17 @@ class DecisionPointDesc(C.Structure):
 
 # FfnDecisionPoint, as a numpy record so that the output array is filled in place
 DECISION_POINT_DTYPE = np.dtype([('id_a', '<u8'), ('id_b', '<u8'), ('dist', '<f8'), ('point_xyz', '<i8', (3,))])
+
+
+class ResegEvalDesc(C.Structure):
+  _fields_ = [('box_zyx', C.c_int32 * 3), ('voxel_size_zyx', C.c_int32 * 3), ('pair', C.c_int32),
+              ('reserved', C.c_int32), ('num_items', C.c_int64)]
+
+
+# FfnResegStats and FfnResegOverlap, as numpy records so that the output arrays are filled in place
+RESEG_STATS_DTYPE = np.dtype([('n_seg', '<i8', (2,)), ('n_reseg', '<i8', (2,)), ('n_reseg_seg', '<i8', (2, 2)),
+                              ('n_inter', '<i8'), ('n_union', '<i8'), ('max_edt2', '<u8', (4,))])
+RESEG_OVERLAP_DTYPE = np.dtype([('item', '<i8'), ('id', '<u8'), ('num_overlapping', '<i8'), ('num_original', '<i8')])
 
 
 class Counters(C.Structure):
@@ -149,6 +160,7 @@ def load() -> C.CDLL:
   lib.ffn_canvas_device_ptr.argtypes = [p, C.c_int, C.POINTER(p), C.POINTER(C.c_int64)]
   lib.ffn_canvas_add_id_offset.argtypes = [p, C.c_int32]
   lib.ffn_decision_points.argtypes = [C.c_int, C.POINTER(DecisionPointDesc), p, p, C.c_int64, C.POINTER(C.c_int64)]
+  lib.ffn_reseg_eval.argtypes = [C.c_int, C.POINTER(ResegEvalDesc), p, p, p, p, p, p, C.c_int64, C.POINTER(C.c_int64)]
   lib.ffn_selftest_wgmma.argtypes = [C.c_int, C.POINTER(C.c_double), C.c_int]
   for name in EXPORTS:
     if name not in ('ffn_last_error', 'ffn_engine_destroy', 'ffn_canvas_destroy'):

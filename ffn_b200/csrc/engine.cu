@@ -23,6 +23,7 @@
 #undef FFN_PROFILE
 #include "seed_kernels.cuh"
 #include "decision_kernels.cuh"
+#include "reseg_kernels.cuh"
 #include "selftest.cuh"
 
 #include <cub/cub.cuh>
@@ -1582,6 +1583,155 @@ int ffn_decision_points(int device, const FfnDecisionPointDesc* desc, uint64_t* 
   });
   *n_out = (int64_t)npairs;
   std::copy(host.begin(), host.begin() + std::min<int64_t>(cap, (int64_t)npairs), out);
+  return 0;
+}
+
+int ffn_reseg_eval(int device, const FfnResegEvalDesc* desc, const uint64_t* labels, const uint8_t* probs,
+                   const uint64_t* ids, const uint8_t mask_table[256], FfnResegStats* stats_out,
+                   FfnResegOverlap* overlaps_out, int64_t cap, int64_t* n_overlaps) {
+  using rsk::u64;
+  if (!desc || !n_overlaps || !stats_out || cap < 0 || (cap > 0 && !overlaps_out) || desc->num_items < 0 ||
+      (desc->num_items > 0 && (!labels || !probs || !ids || !mask_table)))
+    return fail("bad argument");
+  const int bz = desc->box_zyx[0], by = desc->box_zyx[1], bx = desc->box_zyx[2];
+  if (bz < 1 || by < 1 || bx < 1) return fail("box extent must be positive");
+  const long long nitems = desc->num_items, nbox = (long long)bz * by * bx;
+  const bool pair = desc->pair != 0;
+  if (nitems > 0 && nbox > ((1ll << 31) - 1) / (nitems * (pair ? 4 : 1)))
+    return fail("resegmentation analysis supports batches of fewer than 2^31 mask voxels (four masks per pair item)");
+  const int w[3] = {desc->voxel_size_zyx[0], desc->voxel_size_zyx[1], desc->voxel_size_zyx[2]};
+  unsigned __int128 dmax = 0;   // covers the no-background value, which uses the full z extent
+  for (int a = 0; a < 3; ++a) {
+    if (pair && w[a] < 1) return fail("voxel sizes must be positive integers");
+    const unsigned __int128 e = (unsigned __int128)(pair ? w[a] : 0) * (unsigned __int128)desc->box_zyx[a];
+    dmax += e * e;
+  }
+  if (dmax >= ((unsigned __int128)1 << 63)) return fail("voxel size and box too large for exact 64-bit squared distances");
+  *n_overlaps = 0;
+  if (nitems == 0) return 0;
+  cudaDeviceProp prop{};
+  if (check_device(device, &prop)) return 1;
+  CUDA_OK(cudaSetDevice(device));
+  cudaStream_t st = cudaStreamPerThread;
+  const int blocks = prop.multiProcessorCount * 16;
+  // Items (grid y) x blocks per box (grid x): about 16 resident blocks per SM over the whole batch.
+  const dim3 item_grid((unsigned)std::max<long long>(1, std::min<long long>((nbox + 1023) / 1024,
+                                                                              std::max<long long>(1, blocks / nitems))),
+                       (unsigned)std::min<long long>(nitems, 65535));
+  const size_t n = (size_t)(nitems * nbox);
+  const int nprob = pair ? 2 : 1;
+  DevBufs bufs;
+  u64 *d_lab = nullptr, *d_ids = nullptr, *d_counts = nullptr;
+  unsigned char *d_probs = nullptr, *d_table = nullptr;
+  const int ncounts = pair ? rsk::kPairCounts : 2;
+  if (bufs.get(&d_lab, n) || bufs.get(&d_probs, n * nprob) || bufs.get(&d_table, 256) ||
+      bufs.get(&d_counts, (size_t)nitems * ncounts) || bufs.get(&d_ids, 2 * nitems))
+    return 1;
+  CUDA_OK(cudaMemcpyAsync(d_lab, labels, n * sizeof(u64), cudaMemcpyHostToDevice, st));
+  CUDA_OK(cudaMemcpyAsync(d_ids, ids, 2 * nitems * sizeof(u64), cudaMemcpyHostToDevice, st));
+  CUDA_OK(cudaMemcpyAsync(d_probs, probs, n * nprob, cudaMemcpyHostToDevice, st));
+  CUDA_OK(cudaMemcpyAsync(d_table, mask_table, 256, cudaMemcpyHostToDevice, st));
+  CUDA_OK(cudaMemsetAsync(d_counts, 0, (size_t)nitems * ncounts * sizeof(u64), st));
+  std::vector<u64> counts((size_t)nitems * ncounts);
+  std::memset(stats_out, 0, (size_t)nitems * sizeof(FfnResegStats));
+
+  if (pair) {
+    // Four masks per item, then the exact squared EDT of every mask at once: with a single id, the nearest-id keys of
+    // decision_kernels.cuh are plain squared distances (M = 1).  Boxes are stacked along z for the x and y passes and
+    // seen as (masks, Z, Y * X) for the z pass, so that no line crosses a box.
+    const long long nmasks = 4 * nitems;
+    const size_t nk = (size_t)nmasks * nbox;
+    u64 *keys = nullptr, *keys2 = nullptr, *d_max = nullptr;
+    int *sbuf = nullptr, *tbuf = nullptr;
+    if (bufs.get(&keys, nk) || bufs.get(&keys2, nk) || bufs.get(&sbuf, nk) ||
+        bufs.get(&tbuf, nk) || bufs.get(&d_max, nmasks))
+      return 1;
+    CUDA_OK(cudaMemsetAsync(d_max, 0, nmasks * sizeof(u64), st));
+    rsk::pair_prepare<<<item_grid, 256, 0, st>>>(d_lab, d_probs, d_ids, d_table, nitems, nbox, keys, d_counts);
+    const int zs = (int)(nmasks * bz);
+    dpk::nid_x<<<blocks, 128, 0, st>>>(keys, zs, by, bx, (u64)w[2] * (u64)w[2], 1);
+    dpk::nid_line<<<blocks, 128, 0, st>>>(keys, keys2, 1, zs, by, bx, (u64)w[1] * (u64)w[1], sbuf, tbuf);
+    dpk::nid_line<<<blocks, 128, 0, st>>>(keys2, keys, 1, (int)nmasks, bz, by * bx, (u64)w[0] * (u64)w[0], sbuf, tbuf);
+    const dim3 mask_grid(item_grid.x, (unsigned)std::min<long long>(nmasks, 65535));
+    rsk::edt_max<<<mask_grid, 256, 0, st>>>(keys, nmasks, nbox, d_max);
+    CUDA_OK(cudaGetLastError());
+    std::vector<u64> maxes(nmasks);
+    CUDA_OK(cudaMemcpyAsync(maxes.data(), d_max, nmasks * sizeof(u64), cudaMemcpyDeviceToHost, st));
+    CUDA_OK(cudaMemcpyAsync(counts.data(), d_counts, counts.size() * sizeof(u64), cudaMemcpyDeviceToHost, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    // No voxel outside the mask: scipy's feature transform then points every voxel at (-1, 0, 0).
+    const u64 full = (u64)bz * bz * w[0] * w[0] + (u64)(by - 1) * (by - 1) * w[1] * w[1] +
+                     (u64)(bx - 1) * (bx - 1) * w[2] * w[2];
+    for (long long it = 0; it < nitems; ++it) {
+      const u64* c = &counts[it * rsk::kPairCounts];
+      FfnResegStats& s = stats_out[it];
+      s.n_seg[0] = (int64_t)c[0];
+      s.n_seg[1] = (int64_t)c[1];
+      s.n_reseg[0] = (int64_t)c[2];
+      s.n_reseg[1] = (int64_t)c[3];
+      s.n_reseg_seg[0][0] = (int64_t)c[4];
+      s.n_reseg_seg[0][1] = (int64_t)c[5];
+      s.n_reseg_seg[1][0] = (int64_t)c[6];
+      s.n_reseg_seg[1][1] = (int64_t)c[7];
+      s.n_inter = (int64_t)c[8];
+      s.n_union = (int64_t)c[9];
+      for (int k = 0; k < 4; ++k) s.max_edt2[k] = maxes[4 * it + k] == rsk::kInf ? full : maxes[4 * it + k];
+    }
+    return 0;
+  }
+
+  // Endpoint: |mask| per item, and the voxels of every (item, label) split by mask, by sorting on label and then
+  // (stably) on item.
+  if (nitems >= (1ll << 30)) return fail("too many endpoint items");
+  int ibits = 1;
+  while ((1ll << ibits) < nitems) ++ibits;
+  const int ni = (int)n;
+  u64* d_lab2 = nullptr;
+  unsigned *d_vals = nullptr, *d_vals2 = nullptr, *d_scan = nullptr;
+  unsigned char* d_head = nullptr;
+  int *d_heads = nullptr, *d_num = nullptr;
+  char* d_temp = nullptr;
+  if (bufs.get(&d_lab2, n) || bufs.get(&d_vals, n) || bufs.get(&d_vals2, n) || bufs.get(&d_scan, n) ||
+      bufs.get(&d_head, n) || bufs.get(&d_heads, n) || bufs.get(&d_num, 2))
+    return 1;
+  rsk::endpoint_prepare<<<item_grid, 256, 0, st>>>(d_lab, d_probs, d_ids, d_table, nitems, nbox, d_vals, d_counts);
+  FfnResegOverlap* d_rows = nullptr;   // only sized here: at most one row per voxel
+  size_t tb[5] = {0, 0, 0, 0, 0};
+  CUDA_OK(cub::DeviceRadixSort::SortPairs(nullptr, tb[0], d_lab, d_lab2, d_vals, d_vals2, ni, 0, 64, st));
+  CUDA_OK(cub::DeviceRadixSort::SortPairs(nullptr, tb[1], d_vals2, d_vals, d_lab2, d_lab, ni, 1, 1 + ibits, st));
+  CUDA_OK(cub::DeviceSelect::Flagged(nullptr, tb[2], cub::CountingInputIterator<int>(0), d_head, d_heads, d_num, ni, st));
+  CUDA_OK(cub::DeviceScan::InclusiveSum(nullptr, tb[3], d_vals2, d_scan, ni, st));
+  CUDA_OK(cub::DeviceSelect::If(nullptr, tb[4], d_rows, d_rows, d_num + 1, ni, rsk::Overlapping(), st));
+  if (bufs.get(&d_temp, *std::max_element(tb, tb + 5))) return 1;
+  CUDA_OK(cub::DeviceRadixSort::SortPairs(d_temp, tb[0], d_lab, d_lab2, d_vals, d_vals2, ni, 0, 64, st));
+  CUDA_OK(cub::DeviceRadixSort::SortPairs(d_temp, tb[1], d_vals2, d_vals, d_lab2, d_lab, ni, 1, 1 + ibits, st));
+  // Sorted by (item, label): d_vals = item << 1 | mask, d_lab = label.
+  rsk::run_heads<<<blocks, 256, 0, st>>>(d_vals, d_lab, ni, d_head, d_vals2);
+  CUDA_OK(cub::DeviceSelect::Flagged(d_temp, tb[2], cub::CountingInputIterator<int>(0), d_head, d_heads, d_num, ni, st));
+  CUDA_OK(cub::DeviceScan::InclusiveSum(d_temp, tb[3], d_vals2, d_scan, ni, st));
+  int nruns = 0;
+  CUDA_OK(cudaMemcpyAsync(&nruns, d_num, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaMemcpyAsync(counts.data(), d_counts, counts.size() * sizeof(u64), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+  FfnResegOverlap *d_all = nullptr, *d_kept = nullptr;
+  if (bufs.get(&d_all, nruns) || bufs.get(&d_kept, nruns)) return 1;
+  rsk::run_rows<<<blocks, 256, 0, st>>>(d_heads, nruns, ni, d_vals, d_lab, d_scan, d_all);
+  size_t tb_keep = 0;
+  CUDA_OK(cub::DeviceSelect::If(nullptr, tb_keep, d_all, d_kept, d_num + 1, nruns, rsk::Overlapping(), st));
+  if (tb_keep > tb[4]) return fail("overlap selection needs more temporary storage than planned");
+  CUDA_OK(cub::DeviceSelect::If(d_temp, tb_keep, d_all, d_kept, d_num + 1, nruns, rsk::Overlapping(), st));
+  CUDA_OK(cudaGetLastError());
+  int nkept = 0;
+  CUDA_OK(cudaMemcpyAsync(&nkept, d_num + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+  const int64_t m = std::min<int64_t>(cap, nkept);
+  if (m > 0) CUDA_OK(cudaMemcpyAsync(overlaps_out, d_kept, m * sizeof(FfnResegOverlap), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+  for (long long it = 0; it < nitems; ++it) {
+    stats_out[it].n_seg[0] = (int64_t)counts[2 * it];
+    stats_out[it].n_reseg[0] = (int64_t)counts[2 * it + 1];
+  }
+  *n_overlaps = nkept;
   return 0;
 }
 

@@ -221,10 +221,66 @@ def _inference_file():
   return fd
 
 
+def _resegmentation_file():
+  """ffn/inference/resegmentation.proto:22-113: statistics of resegmentation results."""
+  fd = descriptor_pb2.FileDescriptorProto()
+  fd.name = 'inference/resegmentation.proto'
+  fd.package = 'ffn'
+  fd.syntax = 'proto2'
+  fd.dependency.append('utils/vector.proto')
+
+  m = fd.message_type.add()
+  m.name = 'EndpointResegmentationResult'
+  o = m.nested_type.add()
+  o.name = 'OverlapInfo'
+  _field(o, 'num_overlapping', 1, 'int32')
+  _field(o, 'num_original', 2, 'int32')
+  e = m.nested_type.add()   # what protoc generates for map<uint64, OverlapInfo>
+  e.name = 'OverlapsEntry'
+  e.options.map_entry = True
+  _field(e, 'key', 1, 'uint64')
+  _field(e, 'value', 2, '.ffn.EndpointResegmentationResult.OverlapInfo')
+  _field(m, 'id', 1, 'uint64')
+  _field(m, 'start', 2, '.ffn.proto.Vector3j')
+  _field(m, 'num_voxels', 3, 'int32')
+  _field(m, 'overlaps', 4, '.ffn.EndpointResegmentationResult.OverlapsEntry', repeated=True)
+  _field(m, 'source', 5, '.ffn.EndpointResegmentationResult.OverlapInfo')
+  _field(m, 'segmentation_radius', 6, '.ffn.proto.Vector3j')
+  _field(m, 'tag', 7, 'string')
+
+  m = fd.message_type.add()
+  m.name = 'PairResegmentationResult'
+  s = m.nested_type.add()
+  s.name = 'SegmentResult'
+  _field(s, 'origin', 1, '.ffn.proto.Vector3j')
+  _field(s, 'num_voxels', 2, 'int32')
+  _field(s, 'deleted_voxels', 3, 'int32')
+  _field(s, 'segment_a_consistency', 4, 'float')
+  _field(s, 'segment_b_consistency', 5, 'float')
+  _field(s, 'max_edt', 6, 'float')
+  r = m.nested_type.add()
+  r.name = 'EvalResult'
+  _field(r, 'radius', 1, '.ffn.proto.Vector3j')
+  _field(r, 'iou', 2, 'float')
+  _field(r, 'from_a', 3, '.ffn.PairResegmentationResult.SegmentResult')
+  _field(r, 'from_b', 4, '.ffn.PairResegmentationResult.SegmentResult')
+  _field(r, 'max_edt_a', 5, 'float')
+  _field(r, 'max_edt_b', 6, 'float')
+  _field(r, 'num_voxels_a', 7, 'int32')
+  _field(r, 'num_voxels_b', 8, 'int32')
+  _field(m, 'point', 1, '.ffn.proto.Vector3j')
+  _field(m, 'id_a', 2, 'uint64')
+  _field(m, 'id_b', 3, 'uint64')
+  _field(m, 'segmentation_radius', 4, '.ffn.proto.Vector3j')
+  _field(m, 'tag', 5, 'string')
+  _field(m, 'eval', 6, '.ffn.PairResegmentationResult.EvalResult')
+  return fd
+
+
 def _build():
   pool = descriptor_pool.DescriptorPool()   # private pool: never clashes with a real ffn install
   classes = {}
-  for fd in (_vector_file(), _bounding_box_file(), _inference_file()):
+  for fd in (_vector_file(), _bounding_box_file(), _inference_file(), _resegmentation_file()):
     pool.Add(fd)
     file_desc = pool.FindFileByName(fd.name)
     for name, desc in file_desc.message_types_by_name.items():
@@ -254,3 +310,5 @@ ResegmentationPoint = _CLASSES['ffn.ResegmentationPoint']
 ResegmentationRequest = _CLASSES['ffn.ResegmentationRequest']
 CounterValue = _CLASSES['ffn.CounterValue']
 TaskCounters = _CLASSES['ffn.TaskCounters']
+EndpointResegmentationResult = _CLASSES['ffn.EndpointResegmentationResult']
+PairResegmentationResult = _CLASSES['ffn.PairResegmentationResult']

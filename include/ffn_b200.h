@@ -284,6 +284,43 @@ typedef struct {
 int ffn_decision_points(int device, const FfnDecisionPointDesc* desc, uint64_t* labels, FfnDecisionPoint* out,
                         int64_t cap, int64_t* n_out);
 
+/* ---- resegmentation analysis: evaluate_{pair,endpoint}_resegmentation (ffn/inference/resegmentation_analysis.py:97-260)
+ * A batch of items of one kind whose boxes all have the extent box_zyx, laid out back to back (item-major, C-order
+ * zyx): labels [n][box] uint64 original ids, probs [n][2][box] (pair: the analysis box of both objects) or [n][1][box]
+ * (endpoint: the whole segmentation box) uint8 quantised probabilities, ids [n][2] (id_a, id_b; id_b unused for an
+ * endpoint).  A voxel belongs to a resegmented object where mask_table[q] != 0; the caller builds the table from its
+ * own dequantisation and threshold comparison. */
+typedef struct {
+  int32_t box_zyx[3];
+  int32_t voxel_size_zyx[3];  /* positive integers; pairs only */
+  int32_t pair;               /* 1: pair items, 0: endpoint items */
+  int32_t reserved;
+  int64_t num_items;
+} FfnResegEvalDesc;
+/* Per item.  seg_k = (label == id of object k), reseg_k = mask of probability box k.  max_edt2: the largest exact
+ * squared physical distance to the nearest voxel outside the mask (scipy's distance_transform_edt squared) of seg_0,
+ * seg_1, reseg_0, reseg_1; 0 for an empty mask.  A mask without any voxel outside it in the box gets what scipy
+ * returns there, (Z wz)^2 + ((Y-1) wy)^2 + ((X-1) wx)^2.  Endpoint items fill n_seg[0] and n_reseg[0] only. */
+typedef struct {
+  int64_t n_seg[2];
+  int64_t n_reseg[2];
+  int64_t n_reseg_seg[2][2];  /* [k][j] = |reseg_k & seg_j| */
+  int64_t n_inter, n_union;   /* |reseg_0 & reseg_1|, |reseg_0 | reseg_1| */
+  uint64_t max_edt2[4];
+} FfnResegStats;
+/* Endpoint items: one row per (item, original id) with num_overlapping > 0, in (item, id) order; id 0 included. */
+typedef struct {
+  int64_t item;
+  uint64_t id;
+  int64_t num_overlapping;    /* voxels of the id inside the mask */
+  int64_t num_original;       /* voxels of the id in the box */
+} FfnResegOverlap;
+/* stats_out: [n].  overlaps_out receives the first min(count, cap) rows; *n_overlaps = count (0 for pairs).  Fails
+ * when a squared distance could reach 2^63, or when the batch holds 2^31 or more mask voxels (four masks per pair item). */
+int ffn_reseg_eval(int device, const FfnResegEvalDesc* desc, const uint64_t* labels, const uint8_t* probs,
+                   const uint64_t* ids, const uint8_t mask_table[256], FfnResegStats* stats_out,
+                   FfnResegOverlap* overlaps_out, int64_t cap, int64_t* n_overlaps);
+
 /* Known-answer test of the wgmma descriptors (worst absolute error of each case in out[]; see
  * ffn_b200/csrc/selftest.cuh).  Used by tests, not by the product path. */
 int ffn_selftest_wgmma(int device, double* out, int n_out);
