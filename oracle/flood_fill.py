@@ -38,6 +38,9 @@ class Options:
   disco_seed_threshold: float = 0.0     # proto2 default of an unset float field
   min_boundary_dist: Tuple[int, int, int] = (1, 1, 1)   # z, y, x
   min_segment_size: int = 1000
+  # FaceMaxMovementPolicy's score_threshold (logit space, float64), as set by
+  # InferenceRequest.movement_policy_args; None is get_policy_fn's logit(move_threshold)
+  policy_score_threshold: Optional[float] = None
 
 
 def f32_logit(p: float) -> np.float32:
@@ -152,7 +155,10 @@ class Canvas:
     self.seg_prob = np.zeros(self.shape, dtype=np.uint8) if keep_probability_maps else None
     self.mask = mask            # MovementRestrictor.mask (movement.py:303-314)
     self.seed_mask = seed_mask  # MovementRestrictor.seed_mask (movement.py:290-301)
-    self.policy = FaceMaxPolicy(self, deltas_zyx, policy_threshold(options.move_threshold))
+    score_threshold = options.policy_score_threshold
+    if score_threshold is None:
+      score_threshold = policy_threshold(options.move_threshold)
+    self.policy = FaceMaxPolicy(self, deltas_zyx, float(score_threshold))
     self.max_id = 0
     self.origins: Dict[int, Tuple[Tuple[int, int, int], int]] = {}
     self.overlaps: Dict[int, np.ndarray] = {}
@@ -163,6 +169,7 @@ class Canvas:
     self.trace: List[Tuple[int, int, int]] = []      # every FoV position, in order
     self.history: List[Tuple[int, int, int]] = []    # Canvas.history of the current object
     self.history_deleted: List[int] = []             # Canvas.history_deleted of the current object
+    self.disco_applied: List[bool] = []              # per FoV step (all objects): was the disco merge applied
     self.min_margin = float('inf')                   # closest |value - threshold| of any decision
 
   # -- helpers ------------------------------------------------------------------------------
@@ -204,15 +211,18 @@ class Canvas:
     logits = np.array(self.net(fed, self.image[sel]), dtype=np.float32)
     self.counters['inference-calls'] += 1
 
+    merge = False
     if self.disco_seed_threshold >= 0:
       # Canvas.history_deleted (inference.py:420-422; kept unconditionally here, the reference keeps it
       # under keep_history): float32 old seed against the float64 logit(0.8), raw logits against logit(0.5)
       with np.errstate(invalid='ignore'):
         self.history_deleted.append(int(np.sum((old >= 1.3862943611198908) & (logits < 0.0))))
-      if np.mean(logits >= self.move_threshold) > self.disco_seed_threshold:
+      merge = bool(np.mean(logits >= self.move_threshold) > self.disco_seed_threshold)
+      if merge:
         with np.errstate(invalid='ignore'):
           keep_old = (old < np.float32(0.0)) & (logits > old)   # logit(0.5) == 0
         logits[keep_old] = old[keep_old]
+    self.disco_applied.append(merge)
     self.seed[sel] = logits
     return logits
 

@@ -63,7 +63,10 @@ def _check_canvas(canvas, g, exact_seed=True):
   np.testing.assert_array_equal(canvas.segmentation, g['segmentation'])
   if exact_seed:
     np.testing.assert_array_equal(canvas.seed, g['seed_canvas'])
-    np.testing.assert_array_equal(canvas.seg_prob, g['seg_prob'])
+    if canvas.seg_prob is None:                       # keep_probability_maps=False
+      assert 'seg_prob' not in g
+    else:
+      np.testing.assert_array_equal(canvas.seg_prob, g['seg_prob'])
   else:
     np.testing.assert_allclose(canvas.seed, g['seed_canvas'], atol=2e-3, rtol=0, equal_nan=True)
     assert np.abs(canvas.seg_prob.astype(int) - g['seg_prob'].astype(int)).max() <= 1
@@ -176,6 +179,78 @@ def test_toy_anisotropic_flood_fill_bit_exact(golden_dir):
   canvas.segment_all(g['seeds'])
   _check_canvas(canvas, g, exact_seed=True)
   assert g['trace'].shape[0] > 100
+
+
+def oracle_options(case):
+  """ff.Options of a toy_options_flood_fill.npz case (probability space, as the reference got them)."""
+  o = dict(case['options'])
+  o['min_boundary_dist'] = tuple(o['min_boundary_dist'])
+  if case['movement_policy_args']:
+    o['policy_score_threshold'] = json.loads(case['movement_policy_args'])['score_threshold']
+  return ff.Options(**o)
+
+
+OPTION_CASES = ('default', 'manual', 'disco_off', 'disco_partial', 'disco_never', 'policy_low', 'policy_high',
+                'seg_low_pad_low', 'seg_high_move_high', 'weak_seed', 'small_and_tight')
+
+
+@pytest.mark.parametrize('name', OPTION_CASES)
+def test_toy_flood_fill_at_other_inference_options(golden_dir, name):
+  """segment_all away from the FIB-25 options — the manual's recommended set, the disco merge switched off,
+  on for some steps only, or never applied, a movement-policy threshold below / above the move threshold, low
+  and high segment / move / pad values, a weak initial activation, no boundary distance or size limit and
+  no probability map — against the reference's own runs (tests/golden/make_golden_options.py), including the
+  per-step disco merge decision and Canvas.history / history_deleted of one object."""
+  g = _load(golden_dir, 'toy_options_flood_fill.npz')
+  cases = {c['name']: c for c in json.loads(str(g['cases']))}
+  assert sorted(cases) == sorted(OPTION_CASES)
+  case = cases[name]
+  want = {k.split('__', 1)[1]: g[k] for k in g.files if k.startswith(name + '__')}
+  want['seeds'] = g['seeds']
+  canvas = ff.Canvas(toy_net, toy_image(g['cells']), (33, 33, 33), (8, 8, 8), oracle_options(case),
+                     keep_probability_maps=case['keep_probability_maps'])
+  histories = {}
+  segment_at = canvas.segment_at
+
+  def recording_segment_at(pos):
+    n = segment_at(pos)
+    histories[tuple(int(p) for p in pos)] = (list(canvas.history), list(canvas.history_deleted))
+    return n
+  canvas.segment_at = recording_segment_at
+  canvas.segment_all(g['seeds'])
+  _check_canvas(canvas, want, exact_seed=True)
+  ctr = json.loads(str(want['counters']))
+  for k in ('invalid-weak', 'invalid-small'):
+    assert canvas.counters.get(k, 0) == ctr[k], k
+  np.testing.assert_array_equal(np.asarray(canvas.disco_applied, dtype=bool), want['disco_applied'])
+  history, deleted = histories[tuple(int(v) for v in want['history_start'])]
+  np.testing.assert_array_equal(np.asarray(history, np.int64).reshape(-1, 3), want['history'])
+  np.testing.assert_array_equal(np.asarray(deleted, np.int64), want['history_deleted'])
+
+  # the path each case is there for is reached
+  base = json.loads(str(g['default__counters']))
+  steps = int(canvas.counters['inference-calls'])
+  applied = np.asarray(canvas.disco_applied, dtype=bool)
+  if name == 'default':
+    assert applied.all() and steps >= 30
+  elif name == 'manual':
+    assert len(canvas.origins) >= 3
+  elif name == 'disco_off':
+    assert not applied.any() and len(deleted) == 0 < len(history)
+  elif name == 'disco_partial':
+    assert applied.sum() >= 5 and (~applied).sum() >= 5
+  elif name == 'disco_never':
+    assert not applied.any() and len(deleted) == len(history) > 0
+  elif name == 'policy_low':
+    assert canvas.policy.score_threshold < ff.policy_threshold(case['options']['move_threshold'])
+    assert canvas.counters['skip_threshold'] > base.get('skip_threshold', 0)
+  elif name == 'policy_high':
+    assert canvas.policy.score_threshold > ff.policy_threshold(case['options']['move_threshold'])
+    assert steps < base['inference-calls']
+  elif name == 'weak_seed':
+    assert canvas.counters['seed_got_too_weak'] > 0 and canvas.counters['invalid-weak'] > 0
+  elif name == 'small_and_tight':
+    assert canvas.seg_prob is None and case['options']['min_segment_size'] == 0
 
 
 def test_seed_peaks_edt_restatement_equals_the_definition():
