@@ -29,7 +29,7 @@ SEED_POLICY_KINDS = {'peaks_2d': 0, 'fill_empty': 1, 'max_peaks': 2}   # FFN_SEE
 
 EXPORTS = [
     'ffn_last_error', 'ffn_engine_create', 'ffn_engine_destroy', 'ffn_engine_set_compute_mode', 'ffn_engine_set_chains', 'ffn_engine_set_grid',
-    'ffn_engine_info', 'ffn_engine_profile', 'ffn_engine_trace', 'ffn_predict', 'ffn_canvas_create', 'ffn_canvas_destroy',
+    'ffn_engine_info', 'ffn_engine_profile', 'ffn_engine_trace', 'ffn_face_table', 'ffn_predict', 'ffn_canvas_create', 'ffn_canvas_destroy',
     'ffn_canvas_set_mask', 'ffn_canvas_segment_at', 'ffn_canvas_segment_all',
     'ffn_canvas_update_at', 'ffn_canvas_init_seed', 'ffn_canvas_read', 'ffn_canvas_write',
     'ffn_canvas_policy_state_size', 'ffn_canvas_policy_state_get', 'ffn_canvas_policy_state_set',
@@ -134,6 +134,8 @@ def load() -> C.CDLL:
   lib.ffn_engine_info.argtypes = [p, C.POINTER(C.c_int64)]
   lib.ffn_engine_profile.argtypes = [p, C.POINTER(C.c_int64), C.c_int]
   lib.ffn_engine_trace.argtypes = [p, C.POINTER(C.c_int64), C.c_int64, C.c_int]
+  lib.ffn_face_table.argtypes = [C.POINTER(ModelDesc), C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int64),
+                                 C.POINTER(C.c_int32), C.POINTER(C.c_int64)]
   lib.ffn_predict.argtypes = [p, p, p, C.c_int, p]
   lib.ffn_canvas_create.argtypes = [p, p, C.c_int, i32p, C.c_float, C.c_float, C.POINTER(Options),
                                     C.c_int, C.POINTER(p)]

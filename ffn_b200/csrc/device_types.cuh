@@ -5,6 +5,10 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <string.h>
+
+#include <algorithm>
+#include <vector>
 
 #include "../../include/ffn_b200.h"
 
@@ -65,14 +69,27 @@ struct Weights {
 
 // Buffers shared by all chains (the fp32 / split-fp16 parity modes run one chain at a time).
 constexpr int kTraceEvents = 8, kTraceTiles = 2048, kTraceCta = 1;
+constexpr int kProfSlots = 32;    // cycle counters per profiled CTA (ffn_engine_profile)
 
 // Row geometry of the tensor-core epilogue (Workspace::row_flags), per accumulator row m of a tile: the FoV row
 // r = tile * kTileOut - 1 + m is an output row of this tile inside the FoV, x == 0 (no dx = -1 neighbour), x == fx - 1
 // (no dx = +1 neighbour).  A consumer thread's byte holds its rows m0 (bits 0-3) and m0 + 8 (bits 4-7).
 constexpr unsigned kRowValid = 1, kRowX0 = 2, kRowXLast = 4;
 
+// One voxel of one of the six movement faces (movement.py:42-100; face = 2 * axis + (positive side)): its FoV row and
+// `e`, its C-order index inside the face, the index the policy's first-index arg-max ranks equal scores by.
+struct alignas(8) FaceEntry {
+  int row;
+  int face_e;   // face << 24 | e
+};
+// Slots of the face reduction per chain: the six faces without and with the disco merge (flood_kernel.cuh: face_reduce).
+constexpr int kFaceSlots = 12;
+
 struct Workspace {
   const uint8_t* row_flags;   // [nt][8 warps][8 row groups] kRow* flags of a consumer thread's two rows (row_flags_byte)
+  const FaceEntry* face_tab;  // the face voxels ordered by row (build_face_table)
+  const int* face_first;      // [nt + 1] first entry of every tile's rows
+  unsigned long long* face_best;   // [kMaxChains][kFaceSlots] packed (score, index) maxima of the step just computed (face_key)
   __half* act0_l;      // fp16 lo parts (FFN_COMPUTE_FP16X2_TC): x = hi + lo with hi = fp16(x), lo = fp16(x - hi)
   __half* act_l[2];
   float4* act0_f;      // [1][rows_alloc]  (image, seed, 0, 0)
@@ -80,7 +97,7 @@ struct Workspace {
   float4* res;         // [8][rows_alloc] fp32 residual stream (fp32 mode)
   unsigned* bar;       // grid barrier counter
   int* abort_flag;     // != 0: a wait timed out, everybody bails
-  long long* prof;     // [2][16] cycle counters of CTA 0 and CTA G-1, then [kTraceEvents][kTraceTiles] event times of CTA kTraceCta (profiled build)
+  long long* prof;     // [2][kProfSlots] cycle counters of CTA 0 and CTA G-1, then [kTraceEvents][kTraceTiles] event times of CTA kTraceCta (profiled build)
 };
 
 struct CanvasDev {
@@ -276,7 +293,7 @@ struct KParams {
 //   kOffMisc        s_misc: ints [0, kMaxChains) per-chain step-count accumulators, [7] abort flag copy,
 //                   [8, 8 + kMaxChains) disco flags, [16 + 32 k ...) movement-policy scratch of chain k
 //   kOffRound       s_round: [2 * kMaxChains][8] ints
-//   kOffProf        16 cycle counters (profiled build)
+//   kOffProf        kProfSlots cycle counters (profiled build)
 //   kOffXchg        epilogue exchange (4 KB).  The leader's working copies of the chain states
 //                   (kStateSlot bytes each) and of the scheduler block ALIAS this region: CTA 0 uses them only between
 //                   the grid barrier and the end of leader_round, when no epilogue is running.
@@ -285,7 +302,7 @@ constexpr int kOffMisc = 160;
 constexpr int kMiscAbort = 7, kMiscDisco = 8, kMiscScratch = 16;
 constexpr int kOffRound = kOffMisc + (kMiscScratch + 32 * kMaxChains) * 4;
 constexpr int kOffProf = kOffRound + 2 * kMaxChains * 8 * 4;
-constexpr int kOffXchg = (kOffProf + 16 * 8 + 15) / 16 * 16;
+constexpr int kOffXchg = (kOffProf + kProfSlots * 8 + 15) / 16 * 16;
 constexpr int kXchgBytes = 2 * 8 * 2 * 4 * 8 * 4;   // s_xchg: [2 tile parities][8 warps][2 directions][4 channel pairs][4 lanes][2]
 constexpr int kBarsAreaBytes = kOffXchg + kXchgBytes;
 
@@ -327,6 +344,49 @@ inline unsigned row_flags_of(const Geom& g, int tile, int m) {
 inline uint8_t row_flags_byte(const Geom& g, int tile, int warp, int gq) {
   const int m0 = warp * 16 + gq;
   return (uint8_t)(row_flags_of(g, tile, m0) | row_flags_of(g, tile, m0 + 8) << 4);
+}
+
+// The voxels of the movement faces in the order FaceMaxMovementPolicy enumerates them (a face's two in-face axes in C
+// order: (y, x) for the z faces, (z, x) for y, (z, y) for x; an axis with delta 0 has no faces), sorted by row; an edge
+// or corner row appears once per face it lies on.  first[t] .. first[t + 1] are the entries of tile t's output rows.
+inline void build_face_table(const Geom& g, std::vector<FaceEntry>& tab, std::vector<int>& first) {
+  const int c[3] = {g.fz / 2, g.fy / 2, g.fx / 2}, d[3] = {g.dz, g.dy, g.dx};
+  tab.clear();
+  for (int face = 0; face < 6; ++face) {
+    const int axis = face >> 1, a0 = axis == 0 ? 1 : 0, a1 = axis == 2 ? 1 : 2;
+    if (d[axis] == 0) continue;
+    const int n1 = 2 * d[a1] + 1;
+    for (int e = 0; e < (2 * d[a0] + 1) * n1; ++e) {
+      int zyx[3];
+      zyx[axis] = c[axis] + ((face & 1) ? d[axis] : -d[axis]);
+      zyx[a0] = c[a0] - d[a0] + e / n1;
+      zyx[a1] = c[a1] - d[a1] + e % n1;
+      tab.push_back({zyx[0] * g.pp + zyx[1] * g.xp + zyx[2], face << 24 | e});
+    }
+  }
+  std::stable_sort(tab.begin(), tab.end(), [](const FaceEntry& a, const FaceEntry& b) { return a.row < b.row; });
+  first.assign((size_t)g.nt + 1, 0);
+  for (int t = 0, i = 0; t <= g.nt; ++t) {
+    while (i < (int)tab.size() && tab[i].row < t * kTileOut) ++i;
+    first[t] = i;
+  }
+}
+
+// Arg-max of a face as ONE 64-bit maximum: the score's bits mapped to an order-preserving unsigned in the high word,
+// 0xffffffff - e in the low word, so the larger score wins and, among equal scores, the smaller index — the first
+// index in C order, as numpy's argmax.  -0.0 is packed as +0.0 (they compare equal).  0 = no voxel seen yet.
+__host__ __device__ inline unsigned long long face_key(float score, int e) {
+  if (score == 0.f) score = 0.f;
+  unsigned b;
+  memcpy(&b, &score, 4);
+  b ^= (b >> 31) ? 0xffffffffu : 0x80000000u;
+  return (unsigned long long)b << 32 | (0xffffffffu - (unsigned)e);
+}
+__host__ __device__ inline void face_key_unpack(unsigned long long key, float& score, int& e) {
+  unsigned b = (unsigned)(key >> 32);
+  b ^= (b >> 31) ? 0x80000000u : 0xffffffffu;
+  memcpy(&score, &b, 4);
+  e = (int)(0xffffffffu - (unsigned)key);
 }
 
 __host__ __device__ inline size_t w16_layer_offset_halfs(int layer) {

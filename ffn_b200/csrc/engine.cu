@@ -231,6 +231,7 @@ int launch(FfnEngine* e, FfnCanvas* c, int nchains, const Job& job) {
   CUDA_OK(cudaMemsetAsync(e->ws.abort_flag, 0, sizeof(int), cudaStreamPerThread));
   CUDA_OK(cudaMemsetAsync(e->d_ctl, 0, sizeof(Ctl), cudaStreamPerThread));
   CUDA_OK(cudaMemsetAsync(e->d_round_flag, 0, sizeof(unsigned), cudaStreamPerThread));
+  CUDA_OK(cudaMemsetAsync(e->ws.face_best, 0, sizeof(unsigned long long) * kMaxChains * kFaceSlots, cudaStreamPerThread));
   for (int k = 0; k < kMaxChains; ++k) CUDA_OK(cudaMemsetAsync(e->cws[k].bar, 0, sizeof(unsigned), cudaStreamPerThread));
   void* args[] = {&p};
   CUDA_OK(cudaEventRecord(e->ev0, cudaStreamPerThread));
@@ -487,7 +488,7 @@ int ffn_engine_create(int device, const FfnModelDesc* model, const float* const*
   if (dev_alloc(&ws.res, 8 * ra)) return 1;
   if (dev_alloc(&ws.bar, 1)) return 1;
   if (dev_alloc(&ws.abort_flag, 1)) return 1;
-  if (dev_alloc(&ws.prof, 32 + kTraceEvents * kTraceTiles)) return 1;
+  if (dev_alloc(&ws.prof, 2 * kProfSlots + kTraceEvents * kTraceTiles)) return 1;
   for (void* p : std::vector<void*>{ws.act0_l, ws.act_l[0], ws.act_l[1], ws.act0_f, ws.act_f[0], ws.act_f[1], ws.res,
                                     ws.bar, ws.abort_flag, ws.prof})
     e->owned.push_back(p);
@@ -500,6 +501,21 @@ int ffn_engine_create(int device, const FfnModelDesc* model, const float* const*
     e->owned.push_back(d_flags);
     CUDA_OK(cudaMemcpy(d_flags, flags.data(), flags.size(), cudaMemcpyHostToDevice));
     ws.row_flags = d_flags;
+  }
+  {
+    std::vector<FaceEntry> tab;
+    std::vector<int> first;
+    build_face_table(g, tab, first);
+    FaceEntry* d_tab = nullptr;
+    int* d_first = nullptr;
+    if (dev_alloc(&d_tab, std::max<size_t>(tab.size(), 1))) return 1;
+    if (dev_alloc(&d_first, first.size())) return 1;
+    if (dev_alloc(&ws.face_best, (size_t)kMaxChains * kFaceSlots)) return 1;
+    for (void* p : std::vector<void*>{d_tab, d_first, ws.face_best}) e->owned.push_back(p);
+    CUDA_OK(cudaMemcpy(d_tab, tab.data(), tab.size() * sizeof(FaceEntry), cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMemcpy(d_first, first.data(), first.size() * sizeof(int), cudaMemcpyHostToDevice));
+    ws.face_tab = d_tab;
+    ws.face_first = d_first;
   }
   for (int k = 0; k < kMaxChains; ++k) {   // per-chain step workspace: fp16 operands, raw seed, logits, counters, barrier,
     ChainDev& cw = e->cws[k];              // fp32 residual stream
@@ -600,17 +616,36 @@ int ffn_engine_info(FfnEngine* e, int64_t info[8]) {
   return 0;
 }
 
-int ffn_engine_profile(FfnEngine* e, int64_t out[32], int reset) {
+int ffn_engine_profile(FfnEngine* e, int64_t out[64], int reset) {
   if (!e) return fail("null argument");
   if (!out) {   // (out == NULL): switch the device-side counters on (reset != 0) or off (reset == 0)
     e->profiling = reset != 0;
     return 0;
   }
   if (set_device(e)) return 1;
-  long long h[32];
+  static_assert(2 * kProfSlots == 64, "ffn_engine_profile's out[64]");
+  long long h[2 * kProfSlots];
   CUDA_OK(cudaMemcpy(h, e->ws.prof, sizeof(h), cudaMemcpyDeviceToHost));
-  for (int i = 0; i < 32; ++i) out[i] = h[i];
+  for (int i = 0; i < 2 * kProfSlots; ++i) out[i] = h[i];
   if (reset) CUDA_OK(cudaMemset(e->ws.prof, 0, sizeof(h)));
+  return 0;
+}
+
+int ffn_face_table(const FfnModelDesc* model, int64_t cap, int32_t* entries, int64_t* n_entries, int32_t* tile_first,
+                   int64_t* n_tiles) {
+  if (!model || !n_entries || !n_tiles) return fail("null argument");
+  const Geom g = make_geom(*model);
+  std::vector<FaceEntry> tab;
+  std::vector<int> first;
+  build_face_table(g, tab, first);
+  *n_entries = (int64_t)tab.size();
+  *n_tiles = g.nt;
+  for (size_t i = 0; entries && i < tab.size() && (int64_t)i < cap; ++i) {
+    entries[3 * i] = tab[i].row;
+    entries[3 * i + 1] = tab[i].face_e >> 24;
+    entries[3 * i + 2] = tab[i].face_e & 0xffffff;
+  }
+  if (tile_first) std::copy(first.begin(), first.end(), tile_first);
   return 0;
 }
 
@@ -618,8 +653,8 @@ int ffn_engine_trace(FfnEngine* e, int64_t* out, int64_t n, int reset) {
   if (!e || !out || n < 0 || n > (int64_t)kTraceEvents * kTraceTiles) return fail("bad argument");
   if (set_device(e)) return 1;
   static_assert(sizeof(long long) == sizeof(int64_t), "trace element");
-  CUDA_OK(cudaMemcpy(out, e->ws.prof + 32, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost));
-  if (reset) CUDA_OK(cudaMemset(e->ws.prof + 32, 0, sizeof(long long) * kTraceEvents * kTraceTiles));
+  CUDA_OK(cudaMemcpy(out, e->ws.prof + 2 * kProfSlots, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost));
+  if (reset) CUDA_OK(cudaMemset(e->ws.prof + 2 * kProfSlots, 0, sizeof(long long) * kTraceEvents * kTraceTiles));
   return 0;
 }
 

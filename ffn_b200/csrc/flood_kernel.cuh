@@ -95,11 +95,13 @@ __device__ __forceinline__ CanvasState* chain_state(const Ctx& c, int k) {
 // G contiguous ranges of nt / G or nt / G + 1 tiles, but the nt mod G longer ranges start at a different CTA for
 // every chain (CTA index rotated by k * (nt mod G)): a layer of a chain ends when its slowest CTA is done, and one
 // split shared by all chains would give the same CTAs the extra tile of every chain.  This way no CTA works through
-// more than ceil(K * nt / G) tiles of a K-chain round's layer.  Staging and pasting keep the per-CTA row split
-// [t_begin, t_end).
+// more than ceil(K * nt / G) tiles of a K-chain round's layer.  Where the chains' longer ranges fit into CTAs
+// 1 .. G - 1 they start at CTA 1, so that CTA 0 — which every CTA waits for at the round boundary (leader_round; not
+// in predict, which has no leader) — holds only short ranges.  Staging and pasting keep the per-CTA row split [t_begin, t_end).
 __device__ __forceinline__ void chain_tiles(const Ctx& c, int k, int& tb, int& te) {
   const int nt = c.p->g.nt, base = nt / c.G, extra = nt % c.G;
-  const int q = (c.cta + c.G - (k * extra) % c.G) % c.G;
+  const int spare = (c.p->job.mode != MODE_PREDICT && c.p->nchains * extra <= c.G - 1) ? 1 : 0;
+  const int q = (c.cta + c.G - (spare + k * extra) % c.G) % c.G;
   tb = q * base + min(q, extra);
   te = tb + base + (q < extra ? 1 : 0);
 }
@@ -122,7 +124,7 @@ __device__ __forceinline__ void prof_add(const Ctx& c, int slot, long long dt) {
 // register: the fp16 path has none to spare.
 __device__ __forceinline__ void trace_ev(const Ctx& c, int ev, unsigned idx) {
   long long* trace = c.p->ws.prof;
-  if (trace && c.cta == kTraceCta && idx < (unsigned)kTraceTiles) trace[32 + ev * kTraceTiles + idx] = clock64();
+  if (trace && c.cta == kTraceCta && idx < (unsigned)kTraceTiles) trace[2 * kProfSlots + ev * kTraceTiles + idx] = clock64();
 }
 #else
 __device__ __forceinline__ long long prof_now(const Ctx&) { return 0ll; }
@@ -643,6 +645,52 @@ __device__ __forceinline__ void publish_counts(Ctx& c, int k, int hit) {
   }
 }
 
+// movement.get_scored_move_offsets (movement.py:42-100) needs, per face of the step's FoV, the arg-max of the merged
+// logits (first index in C order).  Every CTA reduces the face voxels among the rows of tiles [tb, te) — logits it has
+// just written itself, stored before a CTA-wide barrier the caller has passed — and folds them into the chain's slots
+// with one atomic maximum of a packed (score, index) key (face_key) per warp and face; the end-of-round grid barrier
+// orders the atomics before the leader's reads, which also reset the slots (leader_round).  Whether the disco merge
+// applies is known only once the step's count is complete, so with disco enabled both variants are reduced.
+// `nwarps` warps (0 .. nwarps - 1) call this, in MODE_SEGMENT only: no movement policy runs in predict / update_at.
+__device__ __forceinline__ void face_reduce(const Ctx& c, int k, int tb, int te, int nwarps) {
+  const KParams& p = *c.p;
+  const int e0 = __ldg(p.ws.face_first + tb), e1 = __ldg(p.ws.face_first + te);
+  if (e0 == e1) return;
+  const long long t0 = prof_now(c);
+  const ChainDev& ch = p.ch[k];
+  const bool both = p.cv.opt.disco_seed_threshold >= 0.f;
+  unsigned long long* slots = p.ws.face_best + k * kFaceSlots;
+  for (int base = e0 + 32 * c.warp; base < e1; base += 32 * nwarps) {
+    const int i = base + c.lane;
+    const bool have = i < e1;
+    int face = 0;
+    unsigned long long key = 0, key_d = 0;
+    if (have) {
+      const int2 en = __ldg(reinterpret_cast<const int2*>(p.ws.face_tab + i));   // FaceEntry: (row, face << 24 | e)
+      face = en.y >> 24;
+      const float v = __ldcg(ch.logits + en.x);
+      key = face_key(v, en.y & 0xffffff);
+      if (both) {
+        const float o = __ldcg(ch.seed_raw[c.round & 1u] + en.x);
+        key_d = face_key((o < 0.f && v > o) ? o : v, en.y & 0xffffff);   // merged_row
+      }
+    }
+    unsigned faces = __reduce_or_sync(0xffffffffu, have ? 1u << face : 0u);
+    while (faces) {
+      const int f = __ffs(faces) - 1;
+      faces &= faces - 1;
+      const bool mine = have && face == f;
+      for (int variant = 0; variant < (both ? 2 : 1); ++variant) {
+        const unsigned long long mk = mine ? (variant ? key_d : key) : 0ull;
+        const unsigned hi = __reduce_max_sync(0xffffffffu, (unsigned)(mk >> 32));
+        const unsigned lo = __reduce_max_sync(0xffffffffu, (unsigned)(mk >> 32) == hi ? (unsigned)mk : 0u);
+        if (c.lane == 0) atomicMax(slots + 6 * variant + f, (unsigned long long)hi << 32 | lo);
+      }
+    }
+  }
+  if (c.tid == 0) prof_add(c, 20, prof_now(c) - t0);
+}
+
 // One round of the conv stacks of the chains in `mask`, as ONE warp-specialised pipeline over the work
 // items (layer, chain, tile) in that order:
 //   warp 8    TMA producer : waits for the chain's split-phase barrier (previous layer complete in every
@@ -781,6 +829,10 @@ __device__ __forceinline__ void layers_pipelined(Ctx& c, unsigned mask) {
         }
         if (layer == nconv - 1) {
           publish_counts(c, k, hit);          // the round ends with a grid barrier: no chain arrival needed
+          if (p.job.mode == MODE_SEGMENT) {   // behind publish_counts' barrier of the consumer warps: their logits are stored
+            chain_tiles(c, k, tb, te);        // formed again: nothing more stays live across the tile loop
+            face_reduce(c, k, tb, te, 8);
+          }
         } else {
           chain_arrive_epi(c, k);
         }
@@ -949,6 +1001,10 @@ __device__ __forceinline__ void layers_blocking(Ctx& c) {
     }
     if (layer + 1 < p.g.nconv) grid_barrier(c);
   }
+  if (p.job.mode == MODE_SEGMENT) {
+    __syncthreads();   // this CTA's logits are stored
+    face_reduce(c, 0, c.t_begin, c.t_end, kThreads / 32);
+  }
 }
 
 // Paste this CTA's rows of chain k's last step into the seed canvas (inference.py:439) / the prediction
@@ -1048,18 +1104,20 @@ __device__ __forceinline__ void push_move(const KParams& p, const LChain& L, flo
 // Policy scratch of chain k in shared memory: score[6] floats, rel[6][3], ok[6].
 __device__ __forceinline__ int* policy_scratch(const Ctx& c, int k) { return c.s_misc + kMiscScratch + 32 * k; }
 
-// movement.get_scored_move_offsets (movement.py:42-100) for ONE face of the step just executed at
-// st->cur: arg-max of the merged logits over the face (first index, C order); one warp, every load of
-// the face in flight at once.
-__device__ __forceinline__ void face_argmax(const Ctx& c, const LChain& L, int face) {
+// One face of movement.get_scored_move_offsets (movement.py:42-100) for the step just executed by chain k, from the
+// maximum the CTAs have reduced (face_reduce): the score, the offset of the arg-max from the FoV centre and whether it
+// reaches the policy's threshold go to the chain's policy scratch, and the slots are cleared for the next step.
+__device__ __forceinline__ void face_pick(const Ctx& c, int k, int face, bool disco) {
   const KParams& p = *c.p;
   const Geom& g = p.g;
-  const ChainDev& ch = p.ch[L.k];
-  int* scr = policy_scratch(c, L.k);
+  int* scr = policy_scratch(c, k);
   float* s_score = reinterpret_cast<float*>(scr);
   int* s_rel = scr + 8;     // [6][3]
   int* s_ok = scr + 26;     // [6]
-  const int cz = g.fz / 2, cy = g.fy / 2, cx = g.fx / 2;
+  unsigned long long* slots = p.ws.face_best + k * kFaceSlots;
+  const unsigned long long key = __ldcg(slots + (disco ? 6 : 0) + face);
+  slots[face] = 0ull;
+  slots[6 + face] = 0ull;
   const int axis = face >> 1;
   const int dax = axis == 0 ? g.dz : (axis == 1 ? g.dy : g.dx);
   const int off = (face & 1) ? dax : -dax;
@@ -1067,65 +1125,22 @@ __device__ __forceinline__ void face_argmax(const Ctx& c, const LChain& L, int f
   const int d0 = axis == 0 ? g.dy : g.dz;
   const int d1 = axis == 2 ? g.dy : g.dx;
   const int n0 = 2 * d0 + 1, n1 = 2 * d1 + 1;
-  const float* lgp = ch.logits;
-  const float* odp = ch.seed_raw[L.par];
   int ok = 0;
   if (dax != 0) {
-    float best = -CUDART_INF_F;
-    int best_i = 0x7fffffff;
-    constexpr int kPerLane = 10;   // 320 >= 17 x 17 face elements: one L2 round trip for a whole face
-    for (int base = c.lane; base < n0 * n1; base += 32 * kPerLane) {
-      float lg[kPerLane], od[kPerLane];
-#pragma unroll
-      for (int u = 0; u < kPerLane; ++u) {
-        const int e = base + 32 * u;
-        lg[u] = 0.f;
-        od[u] = 0.f;
-        if (e < n0 * n1) {
-          const int i0 = e / n1, i1 = e - i0 * n1;
-          const int z = axis == 0 ? cz + off : cz - g.dz + i0;
-          const int y = axis == 0 ? cy - g.dy + i0 : (axis == 1 ? cy + off : cy - g.dy + i1);
-          const int x = axis == 2 ? cx + off : cx - g.dx + i1;
-          const int row = z * g.pp + y * g.xp + x;
-          lg[u] = __ldcg(lgp + row);
-          if (L.disco) od[u] = __ldcg(odp + row);
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < kPerLane; ++u) {
-        const int e = base + 32 * u;
-        if (e < n0 * n1) {
-          float v = lg[u];
-          if (L.disco && od[u] < 0.f && v > od[u]) v = od[u];
-          if (v > best || best_i == 0x7fffffff) {
-            best = v;
-            best_i = e;
-          }
-        }
-      }
-    }
-#pragma unroll
-    for (int s = 16; s > 0; s >>= 1) {
-      const float ov = __shfl_xor_sync(0xffffffffu, best, s);
-      const int oi = __shfl_xor_sync(0xffffffffu, best_i, s);
-      if (oi != 0x7fffffff && (best_i == 0x7fffffff || ov > best || (ov == best && oi < best_i))) {
-        best = ov;
-        best_i = oi;
-      }
-    }
-    if (c.lane == 0) {
-      // movement.py:84-86: skip when score < threshold (float64 compare == f32 compare against
-      // the smallest float32 >= threshold)
-      ok = (best >= p.cv.policy_th_f32) ? 1 : 0;
-      const int i0 = best_i / n1, i1 = best_i - i0 * n1;
-      const int r0 = i0 - n0 / 2, r1 = i1 - n1 / 2;
-      s_score[face] = best;
-      s_rel[3 * face + 0] = axis == 0 ? off : r0;
-      s_rel[3 * face + 1] = axis == 0 ? r0 : (axis == 1 ? off : r1);
-      s_rel[3 * face + 2] = axis == 2 ? off : r1;
-    }
+    float best;
+    int best_i;
+    face_key_unpack(key, best, best_i);
+    // movement.py:84-86: skip when score < threshold (float64 compare == f32 compare against
+    // the smallest float32 >= threshold)
+    ok = (best >= p.cv.policy_th_f32) ? 1 : 0;
+    const int i0 = best_i / n1, i1 = best_i - i0 * n1;
+    const int r0 = i0 - n0 / 2, r1 = i1 - n1 / 2;
+    s_score[face] = best;
+    s_rel[3 * face + 0] = axis == 0 ? off : r0;
+    s_rel[3 * face + 1] = axis == 0 ? r0 : (axis == 1 ? off : r1);
+    s_rel[3 * face + 2] = axis == 2 ? off : r1;
   }
-  if (c.lane == 0) s_ok[face] = ok;
+  s_ok[face] = ok;
 }
 
 // FaceMaxMovementPolicy.update (movement.py:210-222) once the six faces are reduced: lanes 0-5 of ONE warp
@@ -1946,7 +1961,8 @@ __device__ __forceinline__ int chain_advance(const Ctx& c, LChain L, Sched* sc, 
 }
 
 // The round boundary on CTA 0 (all threads): policy + pops of the chains that just stepped in parallel
-// (faces spread over all warps, then one warp per chain), then the scheduler transitions of every chain,
+// (the face maxima the CTAs have reduced are unpacked during the copy-in, then one warp per chain), then the
+// scheduler transitions of every chain,
 // serially and in chain order on warp 0 (deterministic), then the actions of the new round are published.
 // `stepped`: chains that ran a FoV step in the round just finished (staged with parity round-1).
 __device__ __forceinline__ void leader_round(Ctx& c, unsigned stepped) {
@@ -1980,25 +1996,22 @@ __device__ __forceinline__ void leader_round(Ctx& c, unsigned stepped) {
     const int k = c.tid - (kThreads - kMaxChains);
     if (k < K) c.s_misc[kMiscDisco + k] = (((stepped >> k) & 1u) && disco_active(p, k, par)) ? 1 : 0;
   }
-  __syncthreads();
-  // ---- phase A.1: the six faces of every chain that stepped, one warp per (chain, face)
-  const long long t_pol = prof_now(c);
-  if (p.job.mode != MODE_UPDATE_AT) {
-    for (int t = c.warp; t < K * 6; t += kThreads / 32) {
-      const int k = t / 6, f = t - 6 * k;
-      if (!((stepped >> k) & 1u)) continue;
-      LChain L{k, sc->active[k], chain_state(c, k), par, c.s_misc[kMiscDisco + k] != 0};
-      face_argmax(c, L, f);
-    }
+  // the six face maxima of every chain that stepped (reduced by all CTAs before the grid barrier)
+  if (p.job.mode == MODE_SEGMENT && c.tid < K * 6) {
+    const int k = c.tid / 6;
+    if ((stepped >> k) & 1u) face_pick(c, k, c.tid - 6 * k, disco_active(p, k, par));
   }
   __syncthreads();
-  // ---- phase A.2: one warp per chain: queue pushes, bookkeeping, the pop that decides the next step
+  const long long t_pol = prof_now(c);
+  if (c.tid == 0) prof_add(c, 16, t_pol - t_all);
+  // ---- phase A: one warp per chain: queue pushes, bookkeeping, the pop that decides the next step
   if (c.warp < K && ((stepped >> c.warp) & 1u)) {
     LChain L{c.warp, sc->active[c.warp], chain_state(c, c.warp), par, c.s_misc[kMiscDisco + c.warp] != 0};
     if (L.st->phase == PH_AFTER_STEP) after_step(c, L);
   }
-  if (c.tid == 0) prof_add(c, 12, prof_now(c) - t_pol);
   __syncthreads();
+  const long long t_adv = prof_now(c);
+  if (c.tid == 0) prof_add(c, 12, t_adv - t_pol);
   // ---- phase B: warp 0, chains in order
   if (c.warp == 0) {
     if (c.lane == 0) {
@@ -2078,6 +2091,8 @@ __device__ __forceinline__ void leader_round(Ctx& c, unsigned stepped) {
     __syncwarp();
   }
   __syncthreads();
+  const long long t_out = prof_now(c);
+  if (c.tid == 0) prof_add(c, 17, t_out - t_adv);
   for (int i = c.tid; i < K * kStateWords; i += 256) {
     if (c.tid >= 256) break;
     const int k = i / kStateWords, w = i - k * kStateWords;
@@ -2090,6 +2105,7 @@ __device__ __forceinline__ void leader_round(Ctx& c, unsigned stepped) {
   // everything above (ordered by bar.sync) becomes visible before the round is announced
   if (c.tid == 0) {
     sm90::red_release_add(p.round_flag, 1u);
+    prof_add(c, 18, prof_now(c) - t_out);
     prof_add(c, 8, prof_now(c) - t_all);
   }
 }
@@ -2288,7 +2304,7 @@ __global__ void __launch_bounds__(kThreads, 1) ffn_flood_kernel(const __grid_con
   c.prof = nullptr;
   if (FFN_PROFILE && p.ws.prof && (c.cta == 0 || c.cta == c.G - 1)) {
     c.prof = reinterpret_cast<long long*>(smem_raw + L.bars + kOffProf);
-    if (c.tid < 16) c.prof[c.tid] = c.tid == 10 ? -clock64() : 0;   // slot 10 (kernel time) adds the clock at exit
+    if (c.tid < kProfSlots) c.prof[c.tid] = c.tid == 10 ? -clock64() : 0;   // slot 10 (kernel time) adds the clock at exit
   }
 #if FFN_PROFILE
   c.sig_cnt = 0;
@@ -2373,7 +2389,9 @@ __global__ void __launch_bounds__(kThreads, 1) ffn_flood_kernel(const __grid_con
       if (c.tid == 0) prof_add(c, 7, prof_now(c) - t_paste);
       // ---- the leader's decisions for this round
       if (c.tid == 0) {
+        const long long t_flag = prof_now(c);
         spin_until(c, p.round_flag, c.round + 1u, 4);
+        prof_add(c, 19, prof_now(c) - t_flag);
         c.s_misc[kMiscAbort] = sm90::ld_volatile_s32(p.ws.abort_flag);   // one reader: the whole CTA must take the same branch
       }
       __syncthreads();
@@ -2422,7 +2440,7 @@ __global__ void __launch_bounds__(kThreads, 1) ffn_flood_kernel(const __grid_con
 
   if (c.tid == 0) prof_add(c, 10, prof_now(c));
   __syncthreads();
-  if (c.prof && c.tid < 16) p.ws.prof[(c.cta == 0 ? 0 : 16) + c.tid] += c.prof[c.tid];
+  if (c.prof && c.tid < kProfSlots) p.ws.prof[(c.cta == 0 ? 0 : kProfSlots) + c.tid] += c.prof[c.tid];
   // Teardown: no bulk copy may be in flight into this CTA's shared memory at exit (the fp16 path always
   // has the next round's layer-0 weights in flight; only the consumer warps know that barrier's parity).
   if (tc && c.warp == 0 && bit_get(c, 8)) mbar_wait(c, &c.mb_w[0], bit_get(c, 0));

@@ -105,17 +105,19 @@ class Engine:
 
   PROFILE_SLOTS = ('barrier_wait', 'act_tma_wait', 'weight_wait', 'mma', 'unused4', 'epi_body',
                    'stage', 'paste', 'leader', 'steps', 'kernel', 'conv_layers', 'leader_policy', 'leader_pops',
-                   'chain_barrier_wait', 'unused')
+                   'chain_barrier_wait', 'unused', 'leader_copy_in', 'leader_advance', 'leader_copy_out',
+                   'round_flag_wait', 'face_reduce') + ('unused',) * 11
 
   def enable_profiling(self, on: bool = True):
     _lib.check(self._lib.ffn_engine_profile(self._h, None, 1 if on else 0))
 
   def profile(self, reset: bool = True) -> dict:
     """Device cycle counters of CTA 0 and of the last CTA (see ffn_engine_profile)."""
-    buf = (C.c_int64 * 32)()
+    n = len(self.PROFILE_SLOTS)
+    buf = (C.c_int64 * (2 * n))()
     _lib.check(self._lib.ffn_engine_profile(self._h, buf, 1 if reset else 0))
-    return {'cta0': dict(zip(self.PROFILE_SLOTS, [int(v) for v in buf[:16]])),
-            'cta_last': dict(zip(self.PROFILE_SLOTS, [int(v) for v in buf[16:32]]))}
+    return {'cta0': dict(zip(self.PROFILE_SLOTS, [int(v) for v in buf[:n]])),
+            'cta_last': dict(zip(self.PROFILE_SLOTS, [int(v) for v in buf[n:]]))}
 
   def trace(self, reset: bool = True) -> np.ndarray:
     """[8 events][2048 tiles] SM-clock timeline of CTA 1 (see ffn_engine_trace); needs enable_profiling()."""

@@ -135,12 +135,22 @@ int ffn_engine_set_grid(FfnEngine* engine, int num_ctas);
 /* sm count, cooperative grid size, shared memory per CTA, tiles per FoV: info[0..3]. */
 int ffn_engine_info(FfnEngine* engine, int64_t info[8]);
 
-/* Device-side cycle counters of CTA 0 (out[0..15]) and the last CTA (out[16..31]): slot 0 grid-barrier
+/* Device-side cycle counters of CTA 0 (out[0..31]) and the last CTA (out[32..63]): slot 0 grid-barrier
  * wait, 1 activation TMA wait, 2 weight wait, 3 MMAs (issue to completion), 4 unused, 5 epilogue body,
- * 6 stage, 7 paste, 8 leader, 9 steps, 10 kernel, 11 conv layers, 12-14 leader parts, 15 layer-end sync.
+ * 6 stage, 7 paste, 8 leader, 9 steps, 10 kernel, 11 conv layers, 12 leader policy (queue pushes + pops), 13 pops,
+ * 14 chain-barrier wait, 15 unused; the leader by phase: 16 state copy-in + the face maxima, (12: policy
+ * updates + pops), 17 scheduler (chain_advance), 18 state copy-out + release; 19 wait for the leader's round flag,
+ * 20 face reduce; 21-31 unused.
  * Off by default (reading the clock perturbs the critical CTA): ffn_engine_profile(e, NULL, 1) switches
  * the counters on, (e, NULL, 0) off; with out != NULL the counters are returned (and reset if reset). */
-int ffn_engine_profile(FfnEngine* engine, int64_t out[32], int reset);
+int ffn_engine_profile(FfnEngine* engine, int64_t out[64], int reset);
+/* The table the flood kernel reduces the movement policy's six faces from (host only, no device needed): the face
+ * voxels of `model`'s field of view ordered by the kernel's row index, entries[3 i ..] = (row, face = 2 * axis +
+ * (positive side), C-order index inside the face); at most `cap` entries are written (entries may be NULL), their
+ * number goes to *n_entries.  tile_first (NULL or [*n_tiles + 1], call once to learn *n_tiles): first entry of every
+ * 126-row tile.  Debug / tests. */
+int ffn_face_table(const FfnModelDesc* model, int64_t cap, int32_t* entries, int64_t* n_entries, int32_t* tile_first,
+                   int64_t* n_tiles);
 /* Tile timeline of one CTA (CTA 1) recorded while the counters are on: out[e * 2048 + i] = SM clock when event e
  * happened to that role's i-th tile since kernel start (0 producer saw the chain barrier, 1 copies issued,
  * 2 consumers saw the operands, 4 MMAs complete, 6 epilogue done, 7 i-th barrier release by the signal warp; 3 and
