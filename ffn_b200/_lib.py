@@ -29,11 +29,11 @@ SEED_POLICY_KINDS = {'peaks_2d': 0, 'fill_empty': 1, 'max_peaks': 2}   # FFN_SEE
 
 EXPORTS = [
     'ffn_last_error', 'ffn_engine_create', 'ffn_engine_destroy', 'ffn_engine_set_compute_mode', 'ffn_engine_set_chains', 'ffn_engine_set_grid',
-    'ffn_engine_info', 'ffn_engine_profile', 'ffn_engine_trace', 'ffn_face_table', 'ffn_predict', 'ffn_canvas_create', 'ffn_canvas_destroy',
+    'ffn_engine_set_step_chunk', 'ffn_engine_info', 'ffn_engine_profile', 'ffn_engine_trace', 'ffn_face_table', 'ffn_predict', 'ffn_canvas_create', 'ffn_canvas_destroy',
     'ffn_canvas_set_mask', 'ffn_canvas_segment_at', 'ffn_canvas_segment_all',
     'ffn_canvas_update_at', 'ffn_canvas_init_seed', 'ffn_canvas_read', 'ffn_canvas_write',
     'ffn_canvas_policy_state_size', 'ffn_canvas_policy_state_get', 'ffn_canvas_policy_state_set',
-    'ffn_canvas_set_resume', 'ffn_canvas_trace', 'ffn_canvas_seed_peaks', 'ffn_canvas_seed_policy', 'ffn_canvas_set_max_id', 'ffn_canvas_get_counters', 'ffn_canvas_spec_stats', 'ffn_canvas_device_ptr',
+    'ffn_canvas_set_resume', 'ffn_canvas_trace', 'ffn_canvas_seed_peaks', 'ffn_canvas_seed_policy', 'ffn_canvas_set_max_id', 'ffn_canvas_get_counters', 'ffn_canvas_spec_stats', 'ffn_canvas_sched_stats', 'ffn_canvas_device_ptr',
     'ffn_canvas_add_id_offset', 'ffn_decision_points', 'ffn_reseg_eval', 'ffn_selftest_wgmma',
 ]
 
@@ -131,6 +131,7 @@ def load() -> C.CDLL:
   lib.ffn_engine_set_compute_mode.argtypes = [p, C.c_int]
   lib.ffn_engine_set_grid.argtypes = [p, C.c_int]
   lib.ffn_engine_set_chains.argtypes = [p, C.c_int]
+  lib.ffn_engine_set_step_chunk.argtypes = [p, C.c_int64]
   lib.ffn_engine_info.argtypes = [p, C.POINTER(C.c_int64)]
   lib.ffn_engine_profile.argtypes = [p, C.POINTER(C.c_int64), C.c_int]
   lib.ffn_engine_trace.argtypes = [p, C.POINTER(C.c_int64), C.c_int64, C.c_int]
@@ -159,6 +160,7 @@ def load() -> C.CDLL:
   lib.ffn_canvas_set_max_id.argtypes = [p, C.c_int64]
   lib.ffn_canvas_get_counters.argtypes = [p, C.POINTER(Counters)]
   lib.ffn_canvas_spec_stats.argtypes = [p, C.POINTER(C.c_int64)]
+  lib.ffn_canvas_sched_stats.argtypes = [p, C.POINTER(C.c_int64), C.c_int]
   lib.ffn_canvas_device_ptr.argtypes = [p, C.c_int, C.POINTER(p), C.POINTER(C.c_int64)]
   lib.ffn_canvas_add_id_offset.argtypes = [p, C.c_int32]
   lib.ffn_decision_points.argtypes = [C.c_int, C.POINTER(DecisionPointDesc), p, p, C.c_int64, C.POINTER(C.c_int64)]

@@ -191,6 +191,25 @@ struct CanvasState {
   FfnCounters ctr;            // segment_at / update_at: cumulative; segment_all: counters of the object in flight
 };
 
+// How often segment_all's scheduler took each of its transitions (lane 0 of the leader warp counts them; the
+// host reports them through ffn_canvas_sched_stats, in this order).  They say which paths a run exercised.
+struct SchedStats {
+  long long parked;                   // a finished object left its chain to wait for its turn (swap_buffers)
+  long long suspended;                // a run was set aside so that a parked object could commit
+  long long resumed;                  // a suspended run went on
+  long long resume_deferred;          // chain-rounds a run suspended in this round could not go on yet (find_suspended_buf)
+  long long turn_taken;               // a chain turned to its parked object because its turn had come (find_turn_buf)
+  long long early_validated;          // an early run was accepted at its turn
+  long long discard_rejected;         // an early run was thrown away and its seed rejected by the in-order gating
+  long long discard_redone;           // an early run was thrown away and its seed redone in turn
+  long long conflict_unstepped_only;  // a conflict found only among the popped-but-not-stepped trajectory entries
+  long long validated_unstepped;      // early runs validated with unstepped entries in their log
+  long long discarded_unstepped;      // early runs found in conflict with unstepped entries in their log
+  long long idle_buffers_full;        // chain-rounds a finished object could not be parked: every buffer was in use
+  long long snapshot_moves;           // Canvas.seed's last in-turn object moved to the snapshot array (ACT_CLEAR_MOVE)
+  long long owner_lost;               // the seed at the head of the line was marked taken but no buffer held it
+};
+
 // Canvas-wide state of segment_all.  The reference processes seeds strictly one after the other
 // (inference.py:538-683).  Here up to kMaxChains objects are in flight: the one whose turn it is (`owner`,
 // holding seed `commit_idx`) and objects started AHEAD of their turn in private seed arrays.  An object's
@@ -229,6 +248,7 @@ struct Sched {
   int snap_lo[3], snap_hi[3];         // box of the snapshot array holding data (hi exclusive)
   int snap_old_lo[3], snap_old_hi[3]; // previous snapshot box, cleared by the move pass of this round
   FfnCounters ctr;            // committed counters (== the reference's)
+  SchedStats tr;              // transition counters of this segment_all
 };
 
 // Leader -> every CTA, once per round.

@@ -69,6 +69,7 @@ struct FfnEngine {
   CUtensorMap tmap[ffn::kMaxChains][3]{};
   int use_tmap = 0;
   int max_chains = ffn::kMaxChains;       // chains the multi-seed / batched paths may use (ffn_engine_set_chains)
+  long long step_chunk = 1 << 15;         // FoV steps per launch of segment_at / segment_all (ffn_engine_set_step_chunk)
   ffn::Ctl* d_ctl = nullptr;
   unsigned* d_round_flag = nullptr;
   ffn::CanvasState* d_dummy_state = nullptr;   // [kMaxBufs]
@@ -102,6 +103,7 @@ struct FfnCanvas {
   ffn::Sched h_sched{};
   size_t q_cap = 0, traj_cap = 0;
   long long last_spec[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // last segment_all: early runs started / discarded / their steps / steps executed
+  std::vector<int64_t> last_sched;        // last segment_all: ffn_canvas_sched_stats
   void* d_image = nullptr;
   uint8_t* d_mask = nullptr;
   uint8_t* d_seed_mask = nullptr;
@@ -595,6 +597,13 @@ int ffn_engine_set_chains(FfnEngine* e, int max_chains) {
   return 0;
 }
 
+int ffn_engine_set_step_chunk(FfnEngine* e, int64_t steps) {
+  if (!e) return fail("null engine");
+  if (steps < 0) return fail("negative step chunk");
+  e->step_chunk = steps == 0 ? 1 << 15 : steps;
+  return 0;
+}
+
 int ffn_engine_set_compute_mode(FfnEngine* e, int mode) {
   if (!e) return fail("null engine");
   if (mode != FFN_COMPUTE_FP16_TC && mode != FFN_COMPUTE_FP32 && mode != FFN_COMPUTE_FP16X2_TC)
@@ -850,7 +859,7 @@ int ffn_canvas_segment_at(FfnCanvas* c, const int32_t start[3], int reset, int64
   double secs = 0;
   for (;;) {
     const long long done = st.ctr.inference_calls - steps0;
-    long long chunk = 1 << 15;
+    long long chunk = e->step_chunk;
     if (max_steps > 0) chunk = std::min<long long>(chunk, max_steps - done);
     job.step_budget = st.ctr.inference_calls + chunk;
     if (launch(e, c, 1, job)) return 1;
@@ -927,6 +936,7 @@ int ffn_canvas_segment_all(FfnCanvas* c, const int32_t* seeds, int64_t n_seeds, 
   sc.steps_executed = 0;
   sc.spec_runs = sc.spec_discarded = sc.spec_steps_discarded = 0;
   sc.idle_free = sc.idle_wait = 0;
+  sc.tr = SchedStats{};
   const unsigned round0 = sc.round;
   sc.all_done = 0;
   sc.ctr = st.ctr;             // cumulative counters of the canvas; the chains count per object from here on
@@ -974,14 +984,14 @@ int ffn_canvas_segment_all(FfnCanvas* c, const int32_t* seeds, int64_t n_seeds, 
   job.ovl_ids = ovl_ids;
   job.seed_status = d_status;
   double secs = 0;
-  long long launches = 0;
+  long long launches = 0, paused_parked = 0, paused_committing = 0;
   int stuck = 0;
   int rc = 0;
   for (;;) {
     const long long before_steps = sc.steps_executed, before_idx = sc.commit_idx;
     const unsigned before_round = sc.round;
-    job.step_budget = sc.steps_executed + (1 << 15);
-    job.round_cap = 2 * (1 << 15) + 8 * n_seeds + 4096;
+    job.step_budget = sc.steps_executed + e->step_chunk;
+    job.round_cap = 2 * e->step_chunk + 8 * n_seeds + 4096;
     if (launch(e, c, K, job)) {
       cleanup();
       return 1;
@@ -993,6 +1003,19 @@ int ffn_canvas_segment_all(FfnCanvas* c, const int32_t* seeds, int64_t n_seeds, 
       return fail("scheduler state copy failed");
     }
     if (sc.all_done) break;
+    // the launch paused: did it leave objects in flight for the next one to resume?
+    bool parked = false, committing = false;
+    for (int b = 0; b < K * kBufsPerChain; ++b) parked = parked || sc.bkind[b] == 1 || sc.bkind[b] == 2;
+    for (int k = 0; k < K; ++k) {
+      CanvasState s;
+      if (cudaMemcpy(&s, c->d_state + sc.active[k], sizeof(CanvasState), cudaMemcpyDeviceToHost) != cudaSuccess) {
+        cleanup();
+        return fail("state copy failed");
+      }
+      committing = committing || s.phase == PH_FINISHED || s.phase == PH_AFTER_COUNT;
+    }
+    paused_parked += parked;
+    paused_committing += committing;
     if (sc.overflow & 16) stuck = 3;   // the device watchdog tripped
     (void)before_round;
     if (stuck < 3) stuck = (sc.steps_executed == before_steps && sc.commit_idx == before_idx) ? stuck + 1 : 0;
@@ -1067,6 +1090,12 @@ int ffn_canvas_segment_all(FfnCanvas* c, const int32_t* seeds, int64_t n_seeds, 
   c->last_spec[5] = sc.idle_free;
   c->last_spec[6] = sc.idle_wait;
   c->last_spec[7] = K;
+  static_assert(sizeof(SchedStats) % sizeof(long long) == 0, "SchedStats holds counters only");
+  const long long* tr = reinterpret_cast<const long long*>(&sc.tr);
+  c->last_sched.assign(tr, tr + sizeof(SchedStats) / sizeof(long long));
+  c->last_sched.push_back(launches);
+  c->last_sched.push_back(paused_parked);
+  c->last_sched.push_back(paused_committing);
   if (counters_out) *counters_out = st.ctr;
   // single-object calls (segment_at, update_at) work on buffer 0 through chain 0
   for (int k = 0; k < kMaxChains; ++k) sc.active[k] = kBufsPerChain * k;
@@ -1445,6 +1474,12 @@ int ffn_canvas_get_counters(FfnCanvas* c, FfnCounters* out) {
 int ffn_canvas_spec_stats(FfnCanvas* c, int64_t out[8]) {
   if (!c || !out) return fail("null argument");
   for (int i = 0; i < 8; ++i) out[i] = c->last_spec[i];
+  return 0;
+}
+
+int ffn_canvas_sched_stats(FfnCanvas* c, int64_t* out, int n) {
+  if (!c || (n > 0 && !out)) return fail("null argument");
+  for (int i = 0; i < n; ++i) out[i] = i < (int)c->last_sched.size() ? c->last_sched[i] : 0;
   return 0;
 }
 

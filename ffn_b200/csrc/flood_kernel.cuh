@@ -1433,9 +1433,9 @@ __device__ __forceinline__ int gate_seed(const Ctx& c, Sched* sc, long long idx,
 }
 
 // Did any FoV position of the (early) run get a label since it was tested?  Warp-collective.
-__device__ __forceinline__ bool run_conflicts(const Ctx& c, int b, const CanvasState* st) {
+__device__ __forceinline__ bool run_conflicts(const Ctx& c, Sched* sc, int b, const CanvasState* st) {
   const KParams& p = *c.p;
-  bool bad = false;
+  bool bad = false, bad_unstepped = false;
   const long long n = min(st->iters, (long long)p.cv.traj_cap);
   for (long long i = c.lane; i < n; i += 32) {
     const int* t = p.ob[b].traj + 3 * i;
@@ -1444,9 +1444,17 @@ __device__ __forceinline__ bool run_conflicts(const Ctx& c, int b, const CanvasS
   // ... or any position it popped as valid without stepping on it (see warp_pop)
   for (long long i = c.lane; i < min((long long)st->n_unstepped, (long long)p.cv.traj_cap - n); i += 32) {
     const int* t = p.ob[b].traj + 3 * ((long long)p.cv.traj_cap - 1 - i);
-    if (__ldcg(p.cv.seg + cv_index(p.cv, __ldcg(t), __ldcg(t + 1), __ldcg(t + 2))) > 0) bad = true;
+    if (__ldcg(p.cv.seg + cv_index(p.cv, __ldcg(t), __ldcg(t + 1), __ldcg(t + 2))) > 0) bad_unstepped = true;
   }
-  return __any_sync(0xffffffffu, bad);
+  const bool stepped = __any_sync(0xffffffffu, bad), unstepped = __any_sync(0xffffffffu, bad_unstepped);
+  if (c.lane == 0) {
+    if (unstepped && !stepped) sc->tr.conflict_unstepped_only++;
+    if (st->n_unstepped > 0) {
+      if (stepped || unstepped) sc->tr.discarded_unstepped++;
+      else sc->tr.validated_unstepped++;
+    }
+  }
+  return stepped || unstepped;
 }
 
 __device__ __forceinline__ void start_object(CanvasState* st, const Sched* sc, long long idx, int spec, int sz, int sy, int sx) {
@@ -1486,8 +1494,11 @@ __device__ __forceinline__ void advance_pointer(const Ctx& c, const LChain& L, S
         if ((sc->bkind[b] == 1 || sc->bkind[b] == 2) && sc->bseed[b] == i) who = b;
       if (c.lane == 0) sc->owner = who;
       __syncwarp();
-      if (who < 0) {   // cannot happen; do not spin on it
-        if (c.lane == 0) sc->commit_idx = i + 1;
+      if (who < 0) {   // cannot happen; do not spin on it, but count it (owner_lost)
+        if (c.lane == 0) {
+          sc->commit_idx = i + 1;
+          sc->tr.owner_lost++;
+        }
         __syncwarp();
         continue;
       }
@@ -1601,6 +1612,9 @@ __device__ __forceinline__ void swap_buffers(const Ctx& c, LChain& L, Sched* sc,
   for (int w = c.lane; w < kStateWords; w += 32)
     reinterpret_cast<unsigned long long*>(st)[w] = __ldcg(reinterpret_cast<const unsigned long long*>(p.ob[nb].st) + w);
   if (c.lane == 0) {
+    if (kind == 1) sc->tr.parked++;
+    if (kind == 2) sc->tr.suspended++;
+    if (sc->bkind[nb] == 2) sc->tr.resumed++;
     sc->bkind[L.b] = kind;
     sc->bseed[L.b] = kind ? left_seed : -1;
     sc->bround[L.b] = (int)sc->round;
@@ -1657,7 +1671,10 @@ __device__ __forceinline__ int chain_advance(const Ctx& c, LChain L, Sched* sc, 
     if (st->seg_all && (phase == PH_FREE || phase == PH_POP || phase == PH_AFTER_CLEAR || phase == PH_FINISHED)) {
       const int tb = find_turn_buf(sc, L.k);
       if (tb >= 0) {
-        if (c.lane == 0) sc->owner = tb;
+        if (c.lane == 0) {
+          sc->owner = tb;
+          sc->tr.turn_taken++;
+        }
         __syncwarp();
         swap_buffers(c, L, sc, tb);
         continue;
@@ -1702,6 +1719,7 @@ __device__ __forceinline__ int chain_advance(const Ctx& c, LChain L, Sched* sc, 
         if (st->seg_all && st->spec && sc->last_chain == L.b && !sc->last_in_snap && p.snap) {
           act = ACT_CLEAR_MOVE;
           if (c.lane == 0) {
+            sc->tr.snapshot_moves++;
             for (int q = 0; q < 3; ++q) {
               sc->snap_old_lo[q] = sc->snap_lo[q];
               sc->snap_old_hi[q] = sc->snap_hi[q];
@@ -1791,6 +1809,10 @@ __device__ __forceinline__ int chain_advance(const Ctx& c, LChain L, Sched* sc, 
             swap_buffers(c, L, sc, nb);
             continue;
           }
+          if (c.lane == 0) {
+            if (too_early) sc->tr.resume_deferred++;
+            else sc->tr.idle_buffers_full++;
+          }
         }
         return ACT_IDLE;
       }
@@ -1806,7 +1828,13 @@ __device__ __forceinline__ int chain_advance(const Ctx& c, LChain L, Sched* sc, 
           bool too_early;
           int nb = find_suspended_buf(sc, L.k, too_early);
           if (nb < 0 && !too_early) nb = find_empty_buf(sc, L.k);
-          if (nb < 0) return ACT_IDLE;
+          if (nb < 0) {
+            if (c.lane == 0) {
+              if (too_early) sc->tr.resume_deferred++;
+              else sc->tr.idle_buffers_full++;
+            }
+            return ACT_IDLE;
+          }
           swap_buffers(c, L, sc, nb);
           continue;
         }
@@ -1814,7 +1842,7 @@ __device__ __forceinline__ int chain_advance(const Ctx& c, LChain L, Sched* sc, 
       if (st->spec) {
         int sz, sy, sx;
         const int ok = gate_seed(c, sc, st->seed_index, true, sz, sy, sx);   // the reference's gating, now, in order
-        const bool conflict = ok && run_conflicts(c, L.b, st);
+        const bool conflict = ok && run_conflicts(c, sc, L.b, st);
         if (!ok || conflict) {
           if (c.lane == 0) {
             sc->spec_discarded++;
@@ -1822,15 +1850,20 @@ __device__ __forceinline__ int chain_advance(const Ctx& c, LChain L, Sched* sc, 
             FfnCounters zero{};
             st->ctr = zero;
             if (!ok) {
+              sc->tr.discard_rejected++;
               finalize_seed(sc, st);                                  // rejected before it would have started
             } else {
+              sc->tr.discard_redone++;
               start_object(st, sc, st->seed_index, 0, sz, sy, sx);    // redo it in turn
             }
           }
           __syncwarp();
           continue;
         }
-        if (c.lane == 0) st->spec = 0;
+        if (c.lane == 0) {
+          st->spec = 0;
+          sc->tr.early_validated++;
+        }
         __syncwarp();
       }
       // from here on this is the reference's code after segment_at returned (inference.py:593-620)
@@ -1949,7 +1982,10 @@ __device__ __forceinline__ int chain_advance(const Ctx& c, LChain L, Sched* sc, 
           swap_buffers(c, L, sc, nb);
           continue;
         }
-        if (too_early) return ACT_IDLE;
+        if (too_early) {   // suspended in this round: its last paste is still landing
+          if (c.lane == 0) sc->tr.resume_deferred++;
+          return ACT_IDLE;
+        }
       }
       lookahead(c, L, sc);                           // then an object ahead of its turn
       if (st->phase == PH_FREE) return ACT_IDLE;     // nothing to start right now
@@ -1976,7 +2012,7 @@ __device__ __forceinline__ void leader_round(Ctx& c, unsigned stepped) {
                 "the leader's working copies alias the epilogue exchange area");
   const unsigned par = (c.round & 1u) ^ 1u;   // parity the finished round was staged with
   const long long t_all = prof_now(c);
-  // Watchdog: one launch covers at most 2^15 FoV steps (a few seconds).  A launch that is still going after
+  // Watchdog: one launch covers at most the engine's step chunk (2^15 FoV steps by default, a few seconds).  A launch that is still going after
   // 60 s (FFN_B200_WATCHDOG_S; sanitizer runs need more) has stalled; raise the abort flag so that every CTA leaves
   // at this round boundary and the host reports it.
   if (c.tid == 0 && sm90::globaltimer_ns() - c.t_start > (unsigned long long)p.job.watchdog_ns) atomicExch(p.ws.abort_flag, 5);

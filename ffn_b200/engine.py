@@ -93,6 +93,11 @@ class Engine:
     """Objects / patches in flight at once in the persistent kernel (1..4, 0 = default 4); see ffn_engine_set_chains."""
     _lib.check(self._lib.ffn_engine_set_chains(self._h, int(max_chains)))
 
+  def set_step_chunk(self, steps: int):
+    """FoV steps per launch of the persistent kernel in segment_at / segment_all (0 = default 2^15); see
+    ffn_engine_set_step_chunk."""
+    _lib.check(self._lib.ffn_engine_set_step_chunk(self._h, int(steps)))
+
   def set_compute_mode(self, mode: int):
     _lib.check(self._lib.ffn_engine_set_compute_mode(self._h, int(mode)))
     self.compute_mode = int(mode)
@@ -247,6 +252,17 @@ class DeviceCanvas:
     _lib.check(self._lib.ffn_canvas_spec_stats(self._h, buf))
     return dict(zip(('early_runs', 'early_runs_discarded', 'steps_discarded', 'steps_executed', 'rounds',
                      'chain_rounds_free', 'chain_rounds_waiting', 'chains'), [int(v) for v in buf]))
+
+  SCHED_STATS = ('parked', 'suspended', 'resumed', 'resume_deferred', 'turn_taken', 'early_validated', 'discard_rejected',
+                 'discard_redone', 'conflict_unstepped_only', 'validated_unstepped', 'discarded_unstepped',
+                 'idle_buffers_full', 'snapshot_moves', 'owner_lost', 'kernel_launches', 'launches_paused_parked',
+                 'launches_paused_committing')
+
+  def sched_stats(self) -> dict:
+    """Scheduler transitions of the last segment_all (see ffn_canvas_sched_stats)."""
+    buf = (C.c_int64 * len(self.SCHED_STATS))()
+    _lib.check(self._lib.ffn_canvas_sched_stats(self._h, buf, len(buf)))
+    return dict(zip(self.SCHED_STATS, [int(v) for v in buf]))
 
   def set_resume(self, iters: int, min_pos, max_pos):
     _lib.check(self._lib.ffn_canvas_set_resume(self._h, int(iters), _lib.i3(min_pos), _lib.i3(max_pos)))

@@ -127,6 +127,10 @@ int ffn_engine_set_compute_mode(FfnEngine* engine, int compute_mode);
  * ffn_predict (the reference batches FoVs into one session.run, executor.py:266-340).  1 = strictly one
  * object / patch at a time. */
 int ffn_engine_set_chains(FfnEngine* engine, int max_chains);
+/* FoV steps one launch of the persistent kernel may run in ffn_canvas_segment_at / ffn_canvas_segment_all before it
+ * pauses at a round boundary and the host launches it again (0 = the default, 2^15).  A small chunk makes every
+ * object cross launch boundaries: the results do not depend on it. */
+int ffn_engine_set_step_chunk(FfnEngine* engine, int64_t steps);
 /* Number of SMs (CTAs of the cooperative grid) this engine's kernel occupies; 0 = all.  Several engines
  * with disjoint SM budgets (e.g. 3 x 44) driven from different host threads run their persistent kernels
  * CONCURRENTLY on one GPU: the H100 form of the reference's batching across canvases
@@ -260,6 +264,17 @@ int ffn_canvas_get_counters(FfnCanvas* canvas, FfnCounters* out);
  * out[4] rounds of the persistent kernel, out[5] / out[6] chain-rounds spent without an object / waiting for the
  * turn to commit, out[7] chains used. */
 int ffn_canvas_spec_stats(FfnCanvas* canvas, int64_t out[8]);
+/* Scheduler transitions of the last ffn_canvas_segment_all, out[0 .. n) (17 values; unused slots are set to 0):
+ * [0] finished objects parked to wait for their turn, [1] runs suspended so that a parked object could commit,
+ * [2] suspended runs resumed, [3] chain-rounds a run suspended in that same round had to wait before it could go on
+ * (its last paste was still landing), [4] parked objects taken up at their turn, [5] early runs validated, [6] / [7]
+ * early runs discarded and their seed rejected / redone in turn ([6] + [7] == spec_stats out[1]), [8] conflicts found
+ * only among the popped-but-not-stepped trajectory entries, [9] / [10] early runs validated / discarded with such
+ * entries, [11] chain-rounds idle because every buffer of the chain was in use, [12] moves of Canvas.seed's last
+ * in-turn object to the snapshot array, [13] seeds skipped at the head of the line because no buffer held them (never
+ * expected), [14] kernel launches, [15] / [16] launches that paused with a parked or suspended object / with a commit
+ * under way. */
+int ffn_canvas_sched_stats(FfnCanvas* canvas, int64_t* out, int n);
 
 /* Multi-GPU merge helpers (SURVEY.md 8e): raw device pointers for NCCL, and the HBM-bound
  * relabel kernel that adds a rank's ID offset to every label > 0. */
