@@ -1378,10 +1378,12 @@ int ffn_canvas_seed_policy(FfnCanvas* c, const FfnSeedPolicyDesc* desc, const do
   double *keys = nullptr, *m1 = nullptr, *m2 = nullptr, *d_noise = nullptr, *zbuf = nullptr, *d_w = nullptr;
   int *vbuf = nullptr, *d_coords = nullptr;
   unsigned long long* d_cnt = nullptr;   // [0] peaks, [1] / [2] ordered bits of the min / max key, [3] unused
+  unsigned long long* d_smin = nullptr;  // 2-D threshold_abs=None: ordered bits of each z-slice's minimum key
   auto cleanup = [&]() {
     cudaFree(a); cudaFree(b); cudaFree(d); cudaFree(keys); cudaFree(m1); cudaFree(m2); cudaFree(d_noise); cudaFree(zbuf);
-    cudaFree(d_w); cudaFree(vbuf); cudaFree(d_coords); cudaFree(d_cnt);
+    cudaFree(d_w); cudaFree(vbuf); cudaFree(d_coords); cudaFree(d_cnt); cudaFree(d_smin);
   };
+  const bool per_slice_min = is2d && desc->threshold_abs_is_min;
   // EDT scratch: 2-D sweeps only along y (lines (z, x)), 3-D also along z (lines (y, x))
   const int maxdim = is2d ? cv.sy : std::max(cv.sz, cv.sy);
   const size_t maxlines = is2d ? (size_t)cv.sz * cv.sx : std::max((size_t)cv.sy * cv.sx, (size_t)cv.sz * cv.sx);
@@ -1401,6 +1403,7 @@ int ffn_canvas_seed_policy(FfnCanvas* c, const FfnSeedPolicyDesc* desc, const do
     alloc_failed = dev_alloc(&a, n, false) || dev_alloc(&b, n, false) || dev_alloc(&d_w, w.size(), false);
   if (!alloc_failed && needs_edt)
     alloc_failed = dev_alloc(&vbuf, (size_t)maxdim * maxlines, false) || dev_alloc(&zbuf, 2 * (size_t)maxdim * maxlines, false);
+  if (!alloc_failed && per_slice_min) alloc_failed = dev_alloc(&d_smin, (size_t)cv.sz, false);
   if (alloc_failed) {
     cleanup();
     return 1;
@@ -1409,6 +1412,7 @@ int ffn_canvas_seed_policy(FfnCanvas* c, const FfnSeedPolicyDesc* desc, const do
   const unsigned long long cnt_init[3] = {0ull, ~0ull, 0ull};
   bool ok = cudaMemcpyAsync(d_cnt, cnt_init, sizeof(cnt_init), cudaMemcpyHostToDevice, st) == cudaSuccess;
   if (noise) ok = ok && cudaMemcpyAsync(d_noise, noise, noise_n * sizeof(double), cudaMemcpyHostToDevice, st) == cudaSuccess;
+  if (per_slice_min) ok = ok && cudaMemsetAsync(d_smin, 0xff, (size_t)cv.sz * sizeof(unsigned long long), st) == cudaSuccess;
   if (desc->kind == FFN_SEED_PEAKS_2D) {
     ok = ok && cudaMemcpyAsync(d_w, w.data(), w.size() * sizeof(double), cudaMemcpyHostToDevice, st) == cudaSuccess;
     seedk::sobel_mag2d<<<blocks, 256, 0, st>>>(cv.image, cv.image_is_u8, cv.mean, cv.stddev, a, cv.sz, cv.sy, cv.sx);
@@ -1430,12 +1434,13 @@ int ffn_canvas_seed_policy(FfnCanvas* c, const FfnSeedPolicyDesc* desc, const do
   }
   const int r = desc->min_distance, rz = is2d ? 0 : r;
   seedk::peak_keys<<<blocks, 256, 0, st>>>(d, d_noise, noise ? noise_n : 0, keys, n, d_cnt + 1);
+  if (per_slice_min) seedk::slice_min_keys<<<cv.sz, 256, 0, st>>>(keys, (size_t)cv.sy * cv.sx, d_smin);
   seedk::box_max<<<blocks, 256, 0, st>>>(keys, m1, r, 2, cv.sz, cv.sy, cv.sx);
   seedk::box_max<<<blocks, 256, 0, st>>>(m1, m2, r, 1, cv.sz, cv.sy, cv.sx);
   if (rz > 0) seedk::box_max<<<blocks, 256, 0, st>>>(m2, m1, rz, 0, cv.sz, cv.sy, cv.sx);
   seedk::peaks_select<<<blocks, 256, 0, st>>>(keys, rz > 0 ? m1 : m2, desc->threshold_abs, desc->threshold_abs_is_min,
-                                              desc->use_threshold_rel, desc->threshold_rel, d_cnt + 1, rz, r, r, cv.sz, cv.sy,
-                                              cv.sx, d_coords, (unsigned long long)cap, d_cnt);
+                                              desc->use_threshold_rel, desc->threshold_rel, d_cnt + 1, d_smin, rz, r, r, cv.sz,
+                                              cv.sy, cv.sx, d_coords, (unsigned long long)cap, d_cnt);
   unsigned long long count = 0;
   ok = ok && cudaGetLastError() == cudaSuccess;
   ok = ok && cudaMemcpyAsync(&count, d_cnt, sizeof(count), cudaMemcpyDeviceToHost, st) == cudaSuccess;

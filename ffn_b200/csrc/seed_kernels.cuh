@@ -6,7 +6,9 @@
 //   gauss_pass x3  1-D correlation, radius 33, reflect          8 B/voxel per pass
 //   edges_kernel   edges > threshold, masks                     9 B/voxel
 //   edt_x / edt_line x2  exact squared EDT (two sweeps, then lower envelope of parabolas per line)
-//   peaks_kernel   7x7x7 maximum of (distance, tie-break noise) keys, plateau-free arg-max test
+//   peaks_kernel   7x7x7 maximum of (distance, tie-break noise) keys, plateau-free arg-max test; like
+//                  peak_local_max's default exclude_border=True (seed.py:191) it drops every peak closer than
+//                  3 voxels to the array border on any axis, whatever the canvas margin
 #pragma once
 
 #include <cuda_runtime.h>
@@ -195,17 +197,19 @@ __global__ void finish_dt(float* d, const int* seg, const uint8_t* mask, const u
 }
 
 // peak_local_max(dt + noise * 1e-4, min_distance = 3, threshold_abs = 0): a voxel is a seed iff its key
-// (dt, noise) is the maximum of its 7x7x7 neighbourhood (edge-clamped) and dt + 1e-4 * noise > 0.
+// (dt, noise) is the maximum of its 7x7x7 neighbourhood (edge-clamped), dt + 1e-4 * noise > 0, and it lies at
+// least `radius` voxels from the array border on every axis (exclude_border=True).
 // Comparing (dt, noise) lexicographically equals comparing the float64 sums because distinct dt
 // values differ by far more than 1e-4.
 __global__ void peaks_kernel(const float* dt, const double* noise, int sz, int sy, int sx, int radius, int* coords,
                              unsigned long long cap, unsigned long long* count) {
   const size_t n = (size_t)sz * sy * sx;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int x = (int)(i % sx), y = (int)((i / sx) % sy), z = (int)(i / ((size_t)sx * sy));
+    if (z < radius || z >= sz - radius || y < radius || y >= sy - radius || x < radius || x >= sx - radius) continue;
     const float v = dt[i];
     const double nv = noise ? noise[i] : 0.0;
     if (!((double)v + nv * 1e-4 > 0.0)) continue;
-    const int x = (int)(i % sx), y = (int)((i / sx) % sy), z = (int)(i / ((size_t)sx * sy));
     bool is_max = true;
     for (int dz = -radius; dz <= radius && is_max; ++dz) {
       const int zz = min(max(z + dz, 0), sz - 1);
@@ -241,6 +245,7 @@ __global__ void peaks_kernel(const float* dt, const double* noise, int sz, int s
 //   masked_image     image with excluded voxels set to 0                10-13 B/voxel
 //   edt_x, edt_line  as above (2-D: x and y sweeps only), then dt_finish 8 B/voxel
 //   peak_keys        float64 key = (double)value + noise * 1e-4, min/max 20 B/voxel (12 with a noise plane in L2)
+//   slice_min_keys   2-D threshold_abs=None only: each z-slice's minimum key  8 B/voxel
 //   box_max x2-3     separable (2r+1) maximum of the keys, one axis each 16 B/voxel per pass
 //   peaks_select     key == box maximum, threshold, border              16 B/voxel
 
@@ -326,6 +331,26 @@ __global__ void peak_keys(const float* values, const double* noise, size_t noise
   }
 }
 
+// threshold_abs=None of PolicyPeaks2d: peak_local_max runs once per z-slice (PolicyPeaks2d), so the threshold is
+// each slice's own minimum key.  One block per slice; slice_min[z] (preset to ~0) receives its ordered bits.
+__global__ void slice_min_keys(const double* keys, size_t slice_n, unsigned long long* slice_min) {
+  const double* s = keys + (size_t)blockIdx.x * slice_n;
+  unsigned long long lo = ~0ull;
+  for (size_t i = threadIdx.x; i < slice_n; i += blockDim.x) {
+    const double k = s[i];
+    if (isfinite(k)) {
+      const unsigned long long o = ordered_bits(k);
+      lo = o < lo ? o : lo;
+    }
+  }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) {
+    const unsigned long long l2 = __shfl_down_sync(0xffffffffu, lo, off);
+    lo = l2 < lo ? l2 : lo;
+  }
+  if ((threadIdx.x & 31) == 0 && lo != ~0ull) atomicMin(&slice_min[blockIdx.x], lo);
+}
+
 // One separable pass of ndimage.maximum_filter(size = 2 radius + 1, mode='nearest') along `axis`: with edge
 // clamping the window maximum is the maximum over the window's part inside the array.  Exact (max is
 // associative), so three passes equal the (2r+1)^3 box; 15 cached loads per voxel at radius 7.
@@ -345,18 +370,23 @@ __global__ void box_max(const double* in, double* out, int radius, int axis, int
 }
 
 // peak_local_max by its documented definition: key == maximum of its box, key > max(threshold_abs,
-// threshold_rel * max key) (threshold_abs = the minimum key when abs_is_min), finite, and at least border[a]
-// voxels from the array border on every axis a.  Appends (z, y, x) to coords (up to cap); *count = peaks.
+// threshold_rel * max key) (threshold_abs = the minimum key when abs_is_min; the minimum key of the voxel's z-slice
+// when slice_min is given), finite, and at least border[a] voxels from the array border on every axis a.  Appends
+// (z, y, x) to coords (up to cap); *count = peaks.
 __global__ void peaks_select(const double* keys, const double* boxmax, double threshold_abs, int abs_is_min, int use_rel,
-                             double threshold_rel, const unsigned long long* minmax, int bz, int by, int bx, int sz,
-                             int sy, int sx, int* coords, unsigned long long cap, unsigned long long* count) {
+                             double threshold_rel, const unsigned long long* minmax, const unsigned long long* slice_min,
+                             int bz, int by, int bx, int sz, int sy, int sx, int* coords, unsigned long long cap,
+                             unsigned long long* count) {
   double thr = abs_is_min ? from_ordered_bits(minmax[0]) : threshold_abs;
-  if (use_rel) thr = fmax(thr, __dmul_rn(threshold_rel, from_ordered_bits(minmax[1])));
+  const double thr_rel = use_rel ? __dmul_rn(threshold_rel, from_ordered_bits(minmax[1])) : -CUDART_INF;
+  thr = fmax(thr, thr_rel);
   const size_t n = (size_t)sz * sy * sx;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     const double k = keys[i];
-    if (!(isfinite(k) && k > thr && k == boxmax[i])) continue;
-    const int x = (int)(i % sx), y = (int)((i / sx) % sy), z = (int)(i / ((size_t)sx * sy));
+    const int z = (int)(i / ((size_t)sx * sy));
+    const double t = slice_min ? fmax(from_ordered_bits(slice_min[z]), thr_rel) : thr;
+    if (!(isfinite(k) && k > t && k == boxmax[i])) continue;
+    const int x = (int)(i % sx), y = (int)((i / sx) % sy);
     if (z < bz || z >= sz - bz || y < by || y >= sy - by || x < bx || x >= sx - bx) continue;
     const unsigned long long slot = atomicAdd(count, 1ull);
     if (slot < cap) {

@@ -93,24 +93,6 @@ class BaseSeedPolicy:
     return mask
 
 
-def _peak_local_max(values, min_distance, threshold_abs):
-  """Local maxima of `values` separated by > min_distance (Chebyshev), best first."""
-  size = 2 * min_distance + 1
-  footprint_max = ndimage.maximum_filter(values, size=size, mode='nearest')
-  peaks = (values == footprint_max) & (values > threshold_abs)
-  coords = np.argwhere(peaks)
-  if coords.shape[0] == 0:
-    return coords
-  order = np.argsort(-values[tuple(coords.T)], kind='stable')
-  return coords[order]
-
-
-def _find_peaks(distances, min_distance, threshold_abs=0, threshold_rel=0):
-  del threshold_rel
-  rng = np.random.RandomState(seed=42)   # seed.py:133-139: reproducible tie-break noise
-  return _peak_local_max(distances + rng.rand(*distances.shape) * 1e-4, min_distance, threshold_abs)
-
-
 _NOISE_CACHE = {}
 
 
@@ -143,7 +125,10 @@ class PolicyPeaks(BaseSeedPolicy):
     if is_edge.all():
       return
     dist = _distance_map(is_edge, self.canvas.voxel_size_zyx, self.get_exclusion_mask())
-    peaks = _find_peaks(dist, min_distance=3, threshold_abs=0, threshold_rel=0)
+    noise = _tie_break_noise(tuple(int(v) for v in self.canvas.shape))
+    # peak_local_max(min_distance=3, threshold_abs=0, threshold_rel=0) with its default exclude_border=True:
+    # peaks closer than 3 voxels to the canvas border are dropped (seed.py:191)
+    peaks = _local_peaks(dist + noise * 1e-4, 3, 0, 0)
     self.coords = np.array(sorted(map(tuple, peaks.astype(int).tolist()))).reshape(-1, 3)
 
   def _blocked_voxels(self):

@@ -15,7 +15,8 @@ So this pins everything the reference's OWN code does around them — Sobel magn
 (sigma 49/6, reflect), masks counted as edges, the all-edges early return, the exclusion mask (labels, mask, seed_mask),
 -1 / non-finite handling, the RandomState(42) tie-break noise, the lexicographic re-sort and the border filter of
 `__next__` — and leaves exactly those two definitions unpinned.  Output: policy_peaks_ref.npz (cases iso / aniso /
-masked).
+masked, and the same three volumes with canvas margins below 3, where the border exclusion of peak_local_max alone
+decides which peaks near the array border survive).
 """
 import os
 import sys
@@ -78,6 +79,10 @@ def main():
       ('iso', (44, 52, 60), 3, (1.0, 1.0, 1.0), (1.0, 1.0, 1.0), (6, 6, 6), False),
       ('aniso', (28, 56, 60), 4, (0.5, 1.0, 1.0), (2.0, 1.0, 1.0), (4, 6, 6), False),
       ('masked', (44, 52, 60), 5, (1.0, 1.0, 1.0), (1.0, 1.0, 1.0), (4, 4, 4), True),
+      # canvas margins below min_distance = 3: only peak_local_max's exclude_border removes the border peaks
+      ('iso_m1', (44, 52, 60), 3, (1.0, 1.0, 1.0), (1.0, 1.0, 1.0), (1, 1, 1), False),
+      ('aniso_m2', (28, 56, 60), 4, (0.5, 1.0, 1.0), (2.0, 1.0, 1.0), (2, 1, 2), False),
+      ('masked_m0', (44, 52, 60), 5, (1.0, 1.0, 1.0), (1.0, 1.0, 1.0), (0, 2, 1), True),
   ]
   for name, shape, seed, sigma, voxel, margin, masked in cases:
     vol = voronoi_phantom(shape, seed=seed, sigma=sigma, voxel_size_zyx=voxel, cell_volume=9000.0)

@@ -108,6 +108,27 @@ def test_no_finite_distance_yields_no_seeds():
   assert seed_policies.policy_fill_empty_space(cv.segmentation).shape == (0, 3)
 
 
+_PEAKS_REF = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'policy_peaks_ref.npz')
+with np.load(_PEAKS_REF) as _r:
+  PEAKS_CASES = sorted(k[:-len('_coords')] for k in _r.files if k.endswith('_coords'))
+
+
+@pytest.mark.parametrize('case', PEAKS_CASES)
+def test_host_policy_peaks_equals_reference(case):
+  """The scipy path of PolicyPeaks (a canvas without a device) yields exactly the reference's list
+  (tests/golden/policy_peaks_ref.npz), order included.  The cases with canvas margins below 3 pin the border
+  exclusion of peak_local_max: a peak 1 or 2 voxels from the array border is never a seed."""
+  r = np.load(_PEAKS_REF)
+  get = lambda k: r[case + k] if case + k in r.files else None   # noqa: E731
+  cv = _HostCanvas(_image(r[case + '_volume']), r[case + '_segmentation'], get('_mask'), get('_seed_mask'),
+                   r[case + '_margin'])
+  cv.voxel_size_zyx = tuple(float(v) for v in r[case + '_voxel'])
+  got = np.array([tuple(v) for v in seed.PolicyPeaks(cv)], dtype=np.int64).reshape(-1, 3)
+  want = r[case + '_coords']
+  assert want.shape[0] >= 5
+  np.testing.assert_array_equal(got, want)
+
+
 @pytest.mark.parametrize('threshold_abs,threshold_rel', [(None, None), (None, 0.3), (0.2, None), (-1.0, 0.6)])
 def test_peak_thresholds_follow_peak_local_max(threshold_abs, threshold_rel):
   """threshold_abs=None is the minimum and threshold_rel=None no relative threshold, as in skimage."""
