@@ -34,7 +34,7 @@ EXPORTS = [
     'ffn_canvas_update_at', 'ffn_canvas_init_seed', 'ffn_canvas_read', 'ffn_canvas_write',
     'ffn_canvas_policy_state_size', 'ffn_canvas_policy_state_get', 'ffn_canvas_policy_state_set',
     'ffn_canvas_set_resume', 'ffn_canvas_trace', 'ffn_canvas_seed_peaks', 'ffn_canvas_seed_policy', 'ffn_canvas_set_max_id', 'ffn_canvas_get_counters', 'ffn_canvas_spec_stats', 'ffn_canvas_sched_stats', 'ffn_canvas_device_ptr',
-    'ffn_canvas_add_id_offset', 'ffn_decision_points', 'ffn_reseg_eval', 'ffn_selftest_wgmma',
+    'ffn_canvas_add_id_offset', 'ffn_decision_points', 'ffn_reseg_eval', 'ffn_split_intersection', 'ffn_selftest_wgmma',
 ]
 
 
@@ -165,6 +165,7 @@ def load() -> C.CDLL:
   lib.ffn_canvas_add_id_offset.argtypes = [p, C.c_int32]
   lib.ffn_decision_points.argtypes = [C.c_int, C.POINTER(DecisionPointDesc), p, p, C.c_int64, C.POINTER(C.c_int64)]
   lib.ffn_reseg_eval.argtypes = [C.c_int, C.POINTER(ResegEvalDesc), p, p, p, p, p, p, C.c_int64, C.POINTER(C.c_int64)]
+  lib.ffn_split_intersection.argtypes = [C.c_int, C.c_int64, p, p, C.c_int64]
   lib.ffn_selftest_wgmma.argtypes = [C.c_int, C.POINTER(C.c_double), C.c_int]
   for name in EXPORTS:
     if name not in ('ffn_last_error', 'ffn_engine_destroy', 'ffn_canvas_destroy'):

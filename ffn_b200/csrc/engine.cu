@@ -24,6 +24,7 @@
 #include "seed_kernels.cuh"
 #include "decision_kernels.cuh"
 #include "reseg_kernels.cuh"
+#include "consensus_kernels.cuh"
 #include "selftest.cuh"
 
 #include <cub/cub.cuh>
@@ -1807,6 +1808,121 @@ int ffn_reseg_eval(int device, const FfnResegEvalDesc* desc, const uint64_t* lab
     stats_out[it].n_reseg[0] = (int64_t)counts[2 * it + 1];
   }
   *n_overlaps = nkept;
+  return 0;
+}
+
+namespace {
+struct MaxU64 {
+  __device__ __forceinline__ unsigned long long operator()(unsigned long long x, unsigned long long y) const {
+    return x > y ? x : y;
+  }
+};
+}  // namespace
+
+int ffn_split_intersection(int device, int64_t n, uint64_t* a, const uint64_t* b, int64_t min_size) {
+  using csk::u64;
+  if (n < 0 || (n > 0 && (!a || !b))) return fail("bad argument");
+  if (n >= (1ll << 31)) return fail("split consensus supports volumes of fewer than 2^31 voxels");
+  if (n == 0) return 0;
+  cudaDeviceProp prop{};
+  if (check_device(device, &prop)) return 1;
+  CUDA_OK(cudaSetDevice(device));
+  cudaStream_t st = cudaStreamPerThread;
+  const int blocks = prop.multiProcessorCount * 16;
+  const int ni = (int)n;
+  DevBufs bufs;
+
+  u64 *d_a = nullptr, *d_b = nullptr, *d_tmp = nullptr, *d_max = nullptr;
+  int* d_num = nullptr;
+  char* d_temp = nullptr;
+  if (bufs.get(&d_a, n) || bufs.get(&d_b, n) || bufs.get(&d_tmp, n) || bufs.get(&d_max, 2) || bufs.get(&d_num, 2))
+    return 1;
+  // Temporary storage for every CUB call below, sized for n items (no later call has more).
+  size_t tb[7] = {0, 0, 0, 0, 0, 0, 0};
+  CUDA_OK(cub::DeviceReduce::Max(nullptr, tb[0], d_a, d_max, ni, st));
+  CUDA_OK(cub::DeviceRadixSort::SortKeys(nullptr, tb[1], d_a, d_tmp, ni, 0, 64, st));
+  CUDA_OK(cub::DeviceSelect::Unique(nullptr, tb[2], d_tmp, d_a, d_num, ni, st));
+  CUDA_OK(cub::DeviceRunLengthEncode::Encode(nullptr, tb[3], d_tmp, d_a, (int*)d_b, d_num, ni, st));
+  CUDA_OK(cub::DeviceRadixSort::SortPairs(nullptr, tb[4], d_tmp, d_a, (int*)d_b, (int*)d_b, ni, 0, 64, st));
+  CUDA_OK(cub::DeviceReduce::ReduceByKey(nullptr, tb[5], (unsigned*)d_a, (unsigned*)d_b, d_tmp, d_a, d_num,
+                                         MaxU64(), ni, st));
+  CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, tb[6], (int*)d_a, (int*)d_b, ni, st));
+  if (bufs.get(&d_temp, *std::max_element(tb, tb + 7))) return 1;
+  CUDA_OK(cudaMemcpyAsync(d_a, a, n * sizeof(u64), cudaMemcpyHostToDevice, st));
+  CUDA_OK(cudaMemcpyAsync(d_b, b, n * sizeof(u64), cudaMemcpyHostToDevice, st));
+  CUDA_OK(cub::DeviceReduce::Max(d_temp, tb[0], d_a, d_max, ni, st));
+  CUDA_OK(cub::DeviceReduce::Max(d_temp, tb[0], d_b, d_max + 1, ni, st));
+  u64 maxes[2] = {0, 0};
+  CUDA_OK(cudaMemcpyAsync(maxes, d_max, sizeof(maxes), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+  const u64 max_id = maxes[0];
+
+  // remap_input: sorted unique ids of an array whose ids do not fit in 32 bits, and the +1 shift when 0 is absent.
+  u64* uniq[2] = {nullptr, nullptr};
+  int nuniq[2] = {0, 0};
+  unsigned shift[2] = {0, 0};
+  for (int k = 0; k < 2; ++k) {
+    if (maxes[k] <= 0xffffffffull) continue;
+    CUDA_OK(cub::DeviceRadixSort::SortKeys(d_temp, tb[1], k ? d_b : d_a, d_tmp, ni, 0, 64, st));
+    if (bufs.get(&uniq[k], n)) return 1;
+    CUDA_OK(cub::DeviceSelect::Unique(d_temp, tb[2], d_tmp, uniq[k], d_num, ni, st));
+    u64 first = 0;
+    CUDA_OK(cudaMemcpyAsync(&nuniq[k], d_num, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CUDA_OK(cudaMemcpyAsync(&first, uniq[k], sizeof(u64), cudaMemcpyDeviceToHost, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    shift[k] = first != 0;
+  }
+
+  // Joint keys (kept in d_tmp for the relabel), sorted into d_b, then the unique pairs and their counts.
+  csk::joint_keys<<<blocks, 256, 0, st>>>(d_a, d_b, (size_t)n, uniq[0], nuniq[0], shift[0], uniq[1], nuniq[1],
+                                          shift[1], d_tmp);
+  CUDA_OK(cudaGetLastError());
+  if (uniq[1]) bufs.release(uniq[1]);
+  CUDA_OK(cub::DeviceRadixSort::SortKeys(d_temp, tb[1], d_tmp, d_b, ni, 0, 64, st));
+  u64* d_pairs = nullptr;
+  int* d_counts = nullptr;
+  if (bufs.get(&d_pairs, n) || bufs.get(&d_counts, n)) return 1;
+  CUDA_OK(cub::DeviceRunLengthEncode::Encode(d_temp, tb[3], d_b, d_pairs, d_counts, d_num, ni, st));
+  int np = 0;
+  CUDA_OK(cudaMemcpyAsync(&np, d_num, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+  bufs.release(d_b);
+
+  // Largest overlap per a: the pairs regrouped by a (a-major sort), then a maximum of count << 32 | ~b per a.
+  u64 *d_sw = nullptr, *d_sw2 = nullptr, *d_pack = nullptr, *d_best = nullptr, *d_lab = nullptr;
+  int *d_idx = nullptr, *d_idx2 = nullptr, *d_flags = nullptr, *d_rank = nullptr;
+  unsigned *d_aof = nullptr, *d_ured = nullptr;
+  unsigned char* d_partner = nullptr;
+  if (bufs.get(&d_sw, np) || bufs.get(&d_sw2, np) || bufs.get(&d_pack, np) || bufs.get(&d_best, np) ||
+      bufs.get(&d_lab, np) || bufs.get(&d_idx, np) || bufs.get(&d_idx2, np) || bufs.get(&d_flags, np) ||
+      bufs.get(&d_rank, np) || bufs.get(&d_aof, np) || bufs.get(&d_ured, np) || bufs.get(&d_partner, np))
+    return 1;
+  csk::regroup<<<blocks, 256, 0, st>>>(d_pairs, np, d_sw, d_idx);
+  CUDA_OK(cub::DeviceRadixSort::SortPairs(d_temp, tb[4], d_sw, d_sw2, d_idx, d_idx2, np, 0, 64, st));
+  csk::partner_pack<<<blocks, 256, 0, st>>>(d_sw2, d_idx2, d_counts, np, d_aof, d_pack);
+  CUDA_OK(cub::DeviceReduce::ReduceByKey(d_temp, tb[5], d_aof, d_ured, d_pack, d_best, d_num + 1, MaxU64(), np, st));
+  int nu = 0;
+  CUDA_OK(cudaMemcpyAsync(&nu, d_num + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+  csk::mark_partner<<<blocks, 256, 0, st>>>(d_aof, d_pack, d_idx2, d_ured, d_best, nu, np, d_partner);
+
+  // New ids in key order, then the output id of every pair.
+  csk::pair_flags<<<blocks, 256, 0, st>>>(d_pairs, d_counts, d_partner, np, (long long)min_size, d_flags);
+  CUDA_OK(cub::DeviceScan::ExclusiveSum(d_temp, tb[6], d_flags, d_rank, np, st));
+  int last[2] = {0, 0};
+  CUDA_OK(cudaMemcpyAsync(&last[0], d_flags + np - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaMemcpyAsync(&last[1], d_rank + np - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+  const u64 n_new = (u64)last[0] + (u64)last[1];
+  if (n_new > ~0ull - max_id)
+    return fail("split consensus: max id " + std::to_string(max_id) + " + " + std::to_string(n_new) +
+                " new ids does not fit in 64 bits");
+  csk::pair_labels<<<blocks, 256, 0, st>>>(d_pairs, d_counts, d_partner, d_rank, np, (long long)min_size, uniq[0],
+                                           shift[0], max_id, d_lab);
+  csk::relabel<<<blocks, 256, 0, st>>>(d_tmp, (size_t)n, d_pairs, np, d_lab, d_a);
+  CUDA_OK(cudaGetLastError());
+  CUDA_OK(cudaMemcpyAsync(a, d_a, n * sizeof(u64), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
   return 0;
 }
 

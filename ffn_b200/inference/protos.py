@@ -277,10 +277,32 @@ def _resegmentation_file():
   return fd
 
 
+def _consensus_file():
+  """ffn/inference/consensus.proto:22-36: the request of split consensus."""
+  fd = descriptor_pb2.FileDescriptorProto()
+  fd.name = 'inference/consensus.proto'
+  fd.package = 'ffn'
+  fd.syntax = 'proto2'
+  fd.dependency.extend(['utils/vector.proto', 'inference/inference.proto'])
+
+  m = fd.message_type.add()
+  m.name = 'ConsensusRequest'
+  e = m.enum_type.add()
+  e.name = 'ConsensusType'
+  ev = e.value.add()
+  ev.name, ev.number = 'CONSENSUS_SPLIT', 2
+  _field(m, 'segmentation1', 1, '.ffn.SegmentationSource')
+  _field(m, 'segmentation2', 2, '.ffn.SegmentationSource')
+  _field(m, 'segmentation_output_dir', 3, 'string')
+  _field(m, 'type', 4, 'enum:.ffn.ConsensusRequest.ConsensusType')
+  _field(m, 'split_min_size', 7, 'int32')
+  return fd
+
+
 def _build():
   pool = descriptor_pool.DescriptorPool()   # private pool: never clashes with a real ffn install
   classes = {}
-  for fd in (_vector_file(), _bounding_box_file(), _inference_file(), _resegmentation_file()):
+  for fd in (_vector_file(), _bounding_box_file(), _inference_file(), _resegmentation_file(), _consensus_file()):
     pool.Add(fd)
     file_desc = pool.FindFileByName(fd.name)
     for name, desc in file_desc.message_types_by_name.items():
@@ -312,3 +334,4 @@ CounterValue = _CLASSES['ffn.CounterValue']
 TaskCounters = _CLASSES['ffn.TaskCounters']
 EndpointResegmentationResult = _CLASSES['ffn.EndpointResegmentationResult']
 PairResegmentationResult = _CLASSES['ffn.PairResegmentationResult']
+ConsensusRequest = _CLASSES['ffn.ConsensusRequest']

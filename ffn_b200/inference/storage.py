@@ -5,8 +5,8 @@ Mirrors the parts of ffn/inference/storage.py the inference path touches: `Origi
 `quantize_probability`/`dequantize_probability` (:137-151), `save_subvolume` (:154-171), the path
 layout helpers (:174-241), `get_existing_subvolume_path` (:244-272), `threshold_segmentation`
 (:275-288), `load_origins` (:291-299), `clip_subvolume_to_bounds` (:302-320), `build_mask`
-(:323-411) and `load_segmentation` (:414-488).  File I/O uses the local filesystem (the
-reference goes through `tf.io.gfile`).
+(:323-411), `load_segmentation` (:414-488) and `load_segmentation_from_source` (:491-511).  File I/O
+uses the local filesystem (the reference goes through `tf.io.gfile`).
 """
 
 import collections
@@ -401,6 +401,50 @@ def load_segmentation(segmentation_dir, corner, allow_cpoint=False, threshold=No
       threshold_segmentation(segmentation_dir, corner, output, threshold)
     if min_size:
       segmentation.clear_dust(output, min_size)
+  return output, origins
+
+
+def load_segmentation_from_source(source, corner):
+  """Loads a saved subvolume as a SegmentationSource proto describes it (storage.py:491-511 with :414-488).
+
+  Supports `directory`, `threshold` and `mask`.  Connected-component splitting and size filtering are not available:
+  the source must set `split_cc: false`, and `min_size` must be unset or 0.
+
+  Args:
+    source: SegmentationSource proto
+    corner: (z, y, x) subvolume corner
+
+  Returns:
+    (labels uint64, origins dict); an all-zero segmentation comes back with no origins, as in the reference
+
+  Raises:
+    NotImplementedError: if `split_cc` is unset or true, or `min_size` is above 0
+    ValueError: when the segmentation (or the probability map a threshold needs) cannot be found
+  """
+  if not source.HasField('split_cc') or source.split_cc:
+    raise NotImplementedError('SegmentationSource.split_cc must be set to false: connected-component splitting is '
+                              'not available')
+  if source.min_size:
+    raise NotImplementedError('SegmentationSource.min_size must be unset or 0: size filtering after connected '
+                              'components is not available')
+  target_path = get_existing_subvolume_path(source.directory, corner)
+  if target_path is None:
+    raise ValueError('Segmentation not found, %s, %r.' % (source.directory, corner))
+  with open(target_path, 'rb') as f:
+    data = np.load(f, allow_pickle=True)
+    if 'segmentation' in data:
+      seg = data['segmentation']
+    else:
+      raise ValueError('FFN NPZ file %s does not contain valid segmentation.' % target_path)
+    origins = _load_origins(data, target_path)
+  if not np.any(seg):
+    return np.zeros(seg.shape, dtype=np.uint64), {}
+  output = seg.astype(np.uint64)
+  if source.HasField('threshold'):
+    threshold_segmentation(source.directory, corner, output, source.threshold)
+  if source.HasField('mask'):
+    mask = build_mask(source.mask.masks, corner, seg.shape)
+    output[mask] = 0
   return output, origins
 
 

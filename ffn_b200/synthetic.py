@@ -66,3 +66,35 @@ def interior_seed(volume_u8: np.ndarray, near_zyx, max_radius: int = 24, bright:
       best = (int(zz[k] + lo[0]), int(yy[k] + lo[1]), int(xx[k] + lo[2]))
       break
   return best if best is not None else (z0, y0, x0)
+
+
+def consensus_pair(shape_zyx, seed: int = 3, big_ids: bool = False):
+  """Two uint64 segmentations of the same Voronoi cells that disagree as a forward and a reverse run do.
+
+  The cells of a 64x128x128 phantom are tiled over `shape_zyx` with distinct ids per tile (membranes stay 0).  The
+  first segmentation cuts every cell along one family of parallel planes, the second along another, and the second
+  also merges cells pairwise.  With `big_ids`, the first segmentation's ids are scaled above 2^32.
+  """
+  shape = tuple(int(s) for s in shape_zyx)
+  _, cells = voronoi_phantom((64, 128, 128), seed=seed, cell_volume=20000.0, return_cells=True)
+  ncell = int(cells.max())
+  a = np.zeros(shape, dtype=np.uint64)
+  b = np.zeros(shape, dtype=np.uint64)
+  z, y, x = np.indices(cells.shape, dtype=np.int64)
+  side_a = ((x + 2 * y + 3 * z) // 37) % 2
+  side_b = ((2 * x - y + z + 1000) // 29) % 2
+  t = 0
+  for z0 in range(0, shape[0], 64):
+    for y0 in range(0, shape[1], 128):
+      for x0 in range(0, shape[2], 128):
+        sel = (slice(z0, z0 + 64), slice(y0, y0 + 128), slice(x0, x0 + 128))
+        n = tuple(s.stop - s.start if s.stop <= d else d - s.start for s, d in zip(sel, shape))
+        c = cells[:n[0], :n[1], :n[2]].astype(np.int64)
+        cid = c + t * ncell
+        la = np.where(c > 0, 2 * cid + side_a[:n[0], :n[1], :n[2]], 0).astype(np.uint64)
+        if big_ids:
+          la = np.where(la > 0, la * np.uint64(2**33) + np.uint64(12345), np.uint64(0))
+        a[sel] = la
+        b[sel] = np.where(c > 0, 2 * (cid // 2) + side_b[:n[0], :n[1], :n[2]] + 1, 0).astype(np.uint64)
+        t += 1
+  return a, b

@@ -346,6 +346,14 @@ int ffn_reseg_eval(int device, const FfnResegEvalDesc* desc, const uint64_t* lab
                    const uint64_t* ids, const uint8_t mask_table[256], FfnResegStats* stats_out,
                    FfnResegOverlap* overlaps_out, int64_t cap, int64_t* n_overlaps);
 
+/* ---- split consensus: split_segmentation_by_intersection (ffn/inference/segmentation.py:181-290) ----------------
+ * a, b: host uint64 [n] label arrays of the same shape.  Every overlapping pair (id_a, id_b), in (id_b, id_a) order,
+ * maps to 0 when it has fewer than min_size voxels or id_a == 0; to id_a when id_b is id_a's largest overlap (the
+ * smallest id_b on equal counts); otherwise to the next new id max(a) + 1, max(a) + 2, ...  a is rewritten in place
+ * with the pair ids; b is only read.  Fails, with no approximate answer, when n >= 2^31 or when max(a) plus the number
+ * of new ids does not fit in 64 bits. */
+int ffn_split_intersection(int device, int64_t n, uint64_t* a, const uint64_t* b, int64_t min_size);
+
 /* Known-answer test of the wgmma descriptors (worst absolute error of each case in out[]; see
  * ffn_b200/csrc/selftest.cuh).  Used by tests, not by the product path. */
 int ffn_selftest_wgmma(int device, double* out, int n_out);
