@@ -34,7 +34,8 @@ EXPORTS = [
     'ffn_canvas_update_at', 'ffn_canvas_init_seed', 'ffn_canvas_read', 'ffn_canvas_write',
     'ffn_canvas_policy_state_size', 'ffn_canvas_policy_state_get', 'ffn_canvas_policy_state_set',
     'ffn_canvas_set_resume', 'ffn_canvas_trace', 'ffn_canvas_seed_peaks', 'ffn_canvas_seed_policy', 'ffn_canvas_set_max_id', 'ffn_canvas_get_counters', 'ffn_canvas_spec_stats', 'ffn_canvas_sched_stats', 'ffn_canvas_device_ptr',
-    'ffn_canvas_add_id_offset', 'ffn_decision_points', 'ffn_reseg_eval', 'ffn_split_intersection', 'ffn_selftest_wgmma',
+    'ffn_canvas_add_id_offset', 'ffn_decision_points', 'ffn_reseg_eval', 'ffn_split_intersection', 'ffn_compute_partitions',
+    'ffn_selftest_wgmma',
 ]
 
 
@@ -74,6 +75,19 @@ class DecisionPointDesc(C.Structure):
   _fields_ = [('shape_zyx', C.c_int32 * 3), ('voxel_size_xyz', C.c_int32 * 3), ('use_max_distance', C.c_int32),
               ('reserved', C.c_int32), ('max_distance', C.c_double), ('box_start_zyx', C.c_int32 * 3),
               ('box_size_zyx', C.c_int32 * 3), ('dust_threshold', C.c_int64)]
+
+
+class ExclusionSphere(C.Structure):
+  _fields_ = [('c_xyz', C.c_int64 * 3), ('r2', C.c_int64), ('f_xyz', C.c_double * 3), ('f_r2', C.c_double),
+              ('integer', C.c_int32), ('reserved', C.c_int32)]
+
+
+class PartitionDesc(C.Structure):
+  _fields_ = [('shape_zyx', C.c_int32 * 3), ('lom_radius_zyx', C.c_int32 * 3), ('min_size', C.c_int64),
+              ('thresholds', C.c_void_p), ('n_thresholds', C.c_int32), ('use_whitelist', C.c_int32),
+              ('whitelist', C.c_void_p), ('n_whitelist', C.c_int64), ('spheres', C.c_void_p),
+              ('n_spheres', C.c_int32), ('reserved', C.c_int32), ('scratch_bytes', C.c_int64),
+              ('n_labels_out', C.c_void_p)]
 
 
 # FfnDecisionPoint, as a numpy record so that the output array is filled in place
@@ -166,6 +180,7 @@ def load() -> C.CDLL:
   lib.ffn_decision_points.argtypes = [C.c_int, C.POINTER(DecisionPointDesc), p, p, C.c_int64, C.POINTER(C.c_int64)]
   lib.ffn_reseg_eval.argtypes = [C.c_int, C.POINTER(ResegEvalDesc), p, p, p, p, p, p, C.c_int64, C.POINTER(C.c_int64)]
   lib.ffn_split_intersection.argtypes = [C.c_int, C.c_int64, p, p, C.c_int64]
+  lib.ffn_compute_partitions.argtypes = [C.c_int, C.POINTER(PartitionDesc), p, p, p, p]
   lib.ffn_selftest_wgmma.argtypes = [C.c_int, C.POINTER(C.c_double), C.c_int]
   for name in EXPORTS:
     if name not in ('ffn_last_error', 'ffn_engine_destroy', 'ffn_canvas_destroy'):

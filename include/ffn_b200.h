@@ -354,6 +354,43 @@ int ffn_reseg_eval(int device, const FfnResegEvalDesc* desc, const uint64_t* lab
  * of new ids does not fit in 64 bits. */
 int ffn_split_intersection(int device, int64_t n, uint64_t* a, const uint64_t* b, int64_t min_size);
 
+/* ---- partition map: compute_partitions (compute_partitions.py:115-204) -------------------------------------------
+ * Exclusion sphere, with the values as given: voxel (x, y, z) of the volume is inside when
+ * (x - cx)^2 + (y - cy)^2 + (z - cz)^2 <= r2, in wrapping int64 (c_xyz, r2) when `integer`, else in float64 (f_xyz,
+ * f_r2) summed left to right. */
+typedef struct {
+  int64_t c_xyz[3];
+  int64_t r2;
+  double f_xyz[3];
+  double f_r2;
+  int32_t integer;
+  int32_t reserved;
+} FfnExclusionSphere;
+typedef struct {
+  int32_t shape_zyx[3];
+  int32_t lom_radius_zyx[3];
+  int64_t min_size;              /* non-zero ids with fewer voxels are cleared first (written back); <= 0: none */
+  const double* thresholds;      /* [n_thresholds], in list order */
+  int32_t n_thresholds;
+  int32_t use_whitelist;         /* 1: only ids in whitelist[] are partitioned */
+  const uint64_t* whitelist;     /* [n_whitelist] ids, signed ids by their two's-complement bits */
+  int64_t n_whitelist;
+  const FfnExclusionSphere* spheres;
+  int32_t n_spheres;
+  int32_t reserved;
+  int64_t scratch_bytes;         /* count scratch per group of labels (8 B per grown-box voxel); <= 0: a quarter of
+                                  * the free device memory.  A label larger than the budget gets a group of its own. */
+  int64_t* n_labels_out;         /* optional: the number of labels partitioned (kept after dust and whitelist) */
+} FfnPartitionDesc;
+/* labels: host uint64 [z][y][x], rewritten in place when dust is cleared.  mask: host uint8 [z][y][x] (non-zero =
+ * masked) or NULL.  out: host uint8 [(z - 2 rz)][(y - 2 ry)][(x - 2 rx)] (the VALID region; nothing when an extent is
+ * not positive): 255 where the LOM box holds a masked voxel or the voxel lies in an exclusion sphere; else, at a voxel
+ * of a partitioned label, i + 1 for the first i with count / prod(2r + 1) < thresholds[i] (float64), or
+ * n_thresholds + 1; else 0.  counts: the 256-bin histogram of out.  Fails, with no approximate answer, for 2^31 or
+ * more voxels or a negative radius. */
+int ffn_compute_partitions(int device, const FfnPartitionDesc* desc, uint64_t* labels, const uint8_t* mask,
+                           uint8_t* out, int64_t counts[256]);
+
 /* Known-answer test of the wgmma descriptors (worst absolute error of each case in out[]; see
  * ffn_b200/csrc/selftest.cuh).  Used by tests, not by the product path. */
 int ffn_selftest_wgmma(int device, double* out, int n_out);
