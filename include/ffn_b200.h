@@ -391,6 +391,43 @@ typedef struct {
 int ffn_compute_partitions(int device, const FfnPartitionDesc* desc, uint64_t* labels, const uint8_t* mask,
                            uint8_t* out, int64_t counts[256]);
 
+/* ---- training coordinates: build_coordinates (build_coordinates.py:61-112) -----------------------------------------
+ * One crop of a partition volume: volume[start + (0 .. crop_shape)] on every axis (z, y, x). */
+typedef struct {
+  int32_t shape_zyx[3];          /* the uint8 volume, C order */
+  int32_t crop_start_zyx[3];
+  int32_t crop_shape_zyx[3];     /* fewer than 2^31 voxels in all; an empty crop writes nothing */
+  int32_t reserved;
+  int64_t volume_index;          /* written as the first element of every row */
+} FfnPartitionRowsDesc;
+/* volume: host uint8 [z][y][x].  rows: host int64 [crop voxels][2], of which the first (crop voxels - counts[255])
+ * are written: (volume_index, flat crop index) for every voxel whose value is not 255, grouped by value in ascending
+ * order and in ascending flat order within a value.  counts: the 256-bin histogram of the crop. */
+int ffn_partition_rows(int device, const FfnPartitionRowsDesc* desc, const uint8_t* volume, int64_t* rows,
+                       int64_t counts[256]);
+
+/* One volume of the coordinate records: center = margin + unravel(flat, crop_shape), reversed to (x, y, z). */
+typedef struct {
+  int32_t crop_shape_zyx[3];
+  int32_t margin_zyx[3];         /* not negative */
+  int64_t name_offset;           /* label_volume_name: names[name_offset .. + name_length] */
+  int64_t name_length;
+} FfnCoordinateVolume;
+typedef struct {
+  const FfnCoordinateVolume* volumes;
+  int32_t n_volumes;
+  int32_t reserved;
+  const uint8_t* names;
+  int64_t names_bytes;
+} FfnCoordinateDesc;
+/* rows: host int64 [n_rows][2] of (volume, flat crop index).  out: host bytes [out_capacity]; receives, per row in
+ * order, the TFRecord frame (u64 length | u32 masked CRC-32C | payload | u32 masked CRC-32C, as TFRecordWriter writes
+ * it before compression) of tf.train.Example {center: Int64List [x, y, z], label_volume_name: BytesList [name]} in
+ * protobuf's deterministic encoding.  *out_bytes: the bytes written.  Fails for a row outside the volume table or an
+ * out_capacity below the frames' size (*out_bytes then holds the size needed). */
+int ffn_coordinate_records(int device, const FfnCoordinateDesc* desc, const int64_t* rows, int64_t n_rows,
+                           uint8_t* out, int64_t out_capacity, int64_t* out_bytes);
+
 /* Known-answer test of the wgmma descriptors (worst absolute error of each case in out[]; see
  * ffn_b200/csrc/selftest.cuh).  Used by tests, not by the product path. */
 int ffn_selftest_wgmma(int device, double* out, int n_out);
