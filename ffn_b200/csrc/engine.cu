@@ -130,9 +130,10 @@ struct DevBufs {
   std::vector<void*> p;
   ~DevBufs() { for (void* q : p) cudaFree(q); }
   template <typename T>
-  int get(T** out, size_t count) {
+  int get(T** out, size_t count, bool zero = false) {
     if (dev_alloc(out, count, false)) return 1;
     p.push_back(*out);
+    if (zero) CUDA_OK(cudaMemset(*out, 0, std::max<size_t>(count, 1) * sizeof(T)));
     return 0;
   }
   void release(void* q) {
@@ -141,8 +142,35 @@ struct DevBufs {
   }
 };
 
+// One temporary-storage buffer for all CUB calls of one entry point.  Each call is written once, as a callable
+// (void* temp, size_t& bytes) -> cudaError_t: alloc() queries every call's size (temp == nullptr) and allocates the
+// largest, and run() runs one call against that buffer.  The sizes are queried at the calls' upper bounds on the item
+// count; CUB refuses a run that needs more than it is given.
+struct CubTemp {
+  char* p = nullptr;
+  size_t bytes = 0;
+  template <typename... F>
+  int alloc(DevBufs& bufs, const F&... calls) {
+    if ((size_for(calls) || ...)) return 1;
+    return bufs.get(&p, bytes);
+  }
+  template <typename F>
+  int size_for(const F& call) {
+    size_t b = 0;
+    CUDA_OK(call(nullptr, b));
+    bytes = std::max(bytes, b);
+    return 0;
+  }
+  template <typename F>
+  cudaError_t run(const F& call) const {
+    size_t b = bytes;
+    return call(p, b);
+  }
+};
+
 // The library only contains sm_90a code: every entry point that takes a device index accepts an sm_90 device only.
-int check_device(int device, cudaDeviceProp* prop) {
+// On success the device is the calling thread's current device and *prop holds its properties.
+int use_device(int device, cudaDeviceProp* prop) {
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
     return fail("no CUDA device: libffn_b200 has no CPU fallback");
@@ -151,6 +179,7 @@ int check_device(int device, cudaDeviceProp* prop) {
   if (prop->major != 9 || prop->minor != 0)
     return fail(std::string("device is sm_") + std::to_string(prop->major) + std::to_string(prop->minor) +
                 "; this library only contains sm_90a code");
+  CUDA_OK(cudaSetDevice(device));
   return 0;
 }
 
@@ -402,6 +431,18 @@ int box_copy(FfnCanvas* c, int which, const int32_t lo[3], const int32_t sz[3], 
   return 0;
 }
 
+// Taps of the seed policies' adaptive-threshold gaussian, sigma = 49/6 truncated at 4 sigma (seed.py:160-163,
+// 240-242): w[0] is the centre tap and w.size() - 1 the radius.
+std::vector<double> seed_gauss_weights() {
+  const double sigma = 49.0 / 6.0;
+  const int radius = (int)(4.0 * sigma + 0.5);
+  std::vector<double> w(radius + 1);
+  double sum = 0;
+  for (int k = -radius; k <= radius; ++k) sum += std::exp(-0.5 / (sigma * sigma) * k * k);
+  for (int k = 0; k <= radius; ++k) w[k] = std::exp(-0.5 / (sigma * sigma) * k * k) / sum;
+  return w;
+}
+
 }  // namespace
 
 extern "C" {
@@ -419,10 +460,9 @@ int ffn_engine_create(int device, const FfnModelDesc* model, const float* const*
       return fail("deltas must lie in [0, fov // 2]");
   }
   cudaDeviceProp prop{};
-  if (check_device(device, &prop)) return 1;
+  if (use_device(device, &prop)) return 1;
   std::unique_ptr<FfnEngine> e(new FfnEngine());
   e->device = device;
-  CUDA_OK(cudaSetDevice(device));
   // Built with --default-stream per-thread: every copy / memset / launch of a host thread goes to that
   // thread's own stream, so engines driven from different host threads run concurrently (SM-partitioned
   // cooperative grids, see ffn_engine_set_grid) while each thread's operations stay ordered.
@@ -904,30 +944,18 @@ int ffn_canvas_segment_all(FfnCanvas* c, const int32_t* seeds, int64_t n_seeds, 
     cudaGetLastError();
     K = 1;
   }
+  DevBufs bufs;
   int* d_seeds = nullptr;
   FfnOrigin* d_orig = nullptr;
   FfnOverlap* d_ovl = nullptr;
   int *d_cnt = nullptr, *d_touched = nullptr;
   unsigned char* d_status = nullptr;
   const int ovl_ids = (int)std::min<int64_t>((int64_t)sc.max_id + n_seeds + 2, (int64_t)1 << 30);
-  auto cleanup = [&]() {
-    cudaFree(d_seeds);
-    cudaFree(d_orig);
-    cudaFree(d_ovl);
-    cudaFree(d_cnt);
-    cudaFree(d_touched);
-    cudaFree(d_status);
-  };
-  if (dev_alloc(&d_seeds, (size_t)n_seeds * 3, false) || dev_alloc(&d_orig, (size_t)origins_cap, false) ||
-      dev_alloc(&d_ovl, (size_t)overlaps_cap, false) || dev_alloc(&d_cnt, (size_t)ovl_ids) ||
-      dev_alloc(&d_touched, (size_t)ovl_ids) || dev_alloc(&d_status, (size_t)n_seeds)) {
-    cleanup();
+  if (bufs.get(&d_seeds, (size_t)n_seeds * 3) || bufs.get(&d_orig, (size_t)origins_cap) ||
+      bufs.get(&d_ovl, (size_t)overlaps_cap) || bufs.get(&d_cnt, (size_t)ovl_ids, true) ||
+      bufs.get(&d_touched, (size_t)ovl_ids, true) || bufs.get(&d_status, (size_t)n_seeds, true))
     return 1;
-  }
-  if (n_seeds && cudaMemcpy(d_seeds, seeds, (size_t)n_seeds * 3 * sizeof(int), cudaMemcpyHostToDevice) != cudaSuccess) {
-    cleanup();
-    return fail("seed list copy failed");
-  }
+  if (n_seeds) CUDA_OK(cudaMemcpy(d_seeds, seeds, (size_t)n_seeds * 3 * sizeof(int), cudaMemcpyHostToDevice));
   // ---- scheduler and chain states
   const bool resume = c->resume_pending;   // finish the restored in-flight object first (inference.py:538-550)
   c->resume_pending = false;
@@ -953,10 +981,7 @@ int ffn_canvas_segment_all(FfnCanvas* c, const int32_t* seeds, int64_t n_seeds, 
     sc.bkind[b] = b >= c->nbufs_alloc || b >= K * kBufsPerChain ? -1 : (b % kBufsPerChain == 0 ? 3 : 0);
   }
   std::vector<CanvasState> hs(kMaxBufs);
-  if (cudaMemcpy(hs.data(), c->d_state, sizeof(CanvasState) * kMaxBufs, cudaMemcpyDeviceToHost) != cudaSuccess) {
-    cleanup();
-    return fail("state copy failed");
-  }
+  CUDA_OK(cudaMemcpy(hs.data(), c->d_state, sizeof(CanvasState) * kMaxBufs, cudaMemcpyDeviceToHost));
   hs[0] = st;
   for (int k = 0; k < kMaxBufs; ++k) {
     CanvasState& h = hs[k];
@@ -969,11 +994,8 @@ int ffn_canvas_segment_all(FfnCanvas* c, const int32_t* seeds, int64_t n_seeds, 
     h.phase = (k == 0 && resume) ? PH_POP : PH_FREE;
     if (!(k == 0 && resume)) h.have_cur = 0;
   }
-  if (cudaMemcpy(c->d_state, hs.data(), sizeof(CanvasState) * kMaxBufs, cudaMemcpyHostToDevice) != cudaSuccess ||
-      cudaMemcpy(c->d_sched, &sc, sizeof(Sched), cudaMemcpyHostToDevice) != cudaSuccess) {
-    cleanup();
-    return fail("state upload failed");
-  }
+  CUDA_OK(cudaMemcpy(c->d_state, hs.data(), sizeof(CanvasState) * kMaxBufs, cudaMemcpyHostToDevice));
+  CUDA_OK(cudaMemcpy(c->d_sched, &sc, sizeof(Sched), cudaMemcpyHostToDevice));
   Job job{};
   job.mode = MODE_SEGMENT;
   job.seeds = d_seeds;
@@ -992,35 +1014,24 @@ int ffn_canvas_segment_all(FfnCanvas* c, const int32_t* seeds, int64_t n_seeds, 
   int rc = 0;
   for (;;) {
     const long long before_steps = sc.steps_executed, before_idx = sc.commit_idx;
-    const unsigned before_round = sc.round;
     job.step_budget = sc.steps_executed + e->step_chunk;
     job.round_cap = 2 * e->step_chunk + 8 * n_seeds + 4096;
-    if (launch(e, c, K, job)) {
-      cleanup();
-      return 1;
-    }
+    if (launch(e, c, K, job)) return 1;
     secs += e->last_kernel_seconds;
     ++launches;
-    if (cudaMemcpy(&sc, c->d_sched, sizeof(Sched), cudaMemcpyDeviceToHost) != cudaSuccess) {
-      cleanup();
-      return fail("scheduler state copy failed");
-    }
+    CUDA_OK(cudaMemcpy(&sc, c->d_sched, sizeof(Sched), cudaMemcpyDeviceToHost));
     if (sc.all_done) break;
     // the launch paused: did it leave objects in flight for the next one to resume?
     bool parked = false, committing = false;
     for (int b = 0; b < K * kBufsPerChain; ++b) parked = parked || sc.bkind[b] == 1 || sc.bkind[b] == 2;
     for (int k = 0; k < K; ++k) {
       CanvasState s;
-      if (cudaMemcpy(&s, c->d_state + sc.active[k], sizeof(CanvasState), cudaMemcpyDeviceToHost) != cudaSuccess) {
-        cleanup();
-        return fail("state copy failed");
-      }
+      CUDA_OK(cudaMemcpy(&s, c->d_state + sc.active[k], sizeof(CanvasState), cudaMemcpyDeviceToHost));
       committing = committing || s.phase == PH_FINISHED || s.phase == PH_AFTER_COUNT;
     }
     paused_parked += parked;
     paused_committing += committing;
     if (sc.overflow & 16) stuck = 3;   // the device watchdog tripped
-    (void)before_round;
     if (stuck < 3) stuck = (sc.steps_executed == before_steps && sc.commit_idx == before_idx) ? stuck + 1 : 0;
     if (stuck >= 3) {
       std::vector<CanvasState> dbg(kMaxBufs);
@@ -1077,7 +1088,6 @@ int ffn_canvas_segment_all(FfnCanvas* c, const int32_t* seeds, int64_t n_seeds, 
     if (cudaMemcpy(overlaps_out, d_ovl, (size_t)std::min<long long>(sc.n_overlaps, overlaps_cap) * sizeof(FfnOverlap),
                    cudaMemcpyDeviceToHost) != cudaSuccess)
       rc = fail("overlaps copy failed");
-  cleanup();
   st.ctr = sc.ctr;
   st.ctr.max_id = sc.max_id;
   st.ctr.device_seconds += secs;
@@ -1103,7 +1113,7 @@ int ffn_canvas_segment_all(FfnCanvas* c, const int32_t* seeds, int64_t n_seeds, 
   // single-object calls (segment_at, update_at) work on buffer 0 through chain 0
   for (int k = 0; k < kMaxChains; ++k) sc.active[k] = kBufsPerChain * k;
   sc.owner = -1;
-  if (cudaMemcpy(c->d_sched, &sc, sizeof(Sched), cudaMemcpyHostToDevice) != cudaSuccess) return fail("scheduler state upload failed");
+  CUDA_OK(cudaMemcpy(c->d_sched, &sc, sizeof(Sched), cudaMemcpyHostToDevice));
   if (push_state(c)) return 1;
   return rc;
 }
@@ -1146,13 +1156,12 @@ int ffn_canvas_read(FfnCanvas* c, int which, const int32_t lo[3], const int32_t 
       CUDA_OK(cudaMemcpy(dst, cv.image, c->nvox * 4, cudaMemcpyDeviceToHost));
       return 0;
     }
+    DevBufs bufs;
     float* tmp = nullptr;
-    if (dev_alloc(&tmp, c->nvox, false)) return 1;
+    if (bufs.get(&tmp, c->nvox)) return 1;
     normalize_u8_kernel<<<c->eng->sm_count * 8, 256, 0, cudaStreamPerThread>>>(
         reinterpret_cast<const uint8_t*>(cv.image), tmp, c->nvox, cv.mean, cv.stddev);
-    cudaError_t err = cudaMemcpy(dst, tmp, c->nvox * 4, cudaMemcpyDeviceToHost);
-    cudaFree(tmp);
-    if (err != cudaSuccess) return fail(cudaGetErrorString(err));
+    CUDA_OK(cudaMemcpy(dst, tmp, c->nvox * 4, cudaMemcpyDeviceToHost));
     return 0;
   }
   return box_copy(c, which, lo, sz, dst, true);
@@ -1308,35 +1317,22 @@ int ffn_canvas_seed_peaks(FfnCanvas* c, const float voxel_size_zyx[3], const dou
   const CanvasDev& cv = c->cv;
   const size_t n = c->nvox;
   const int blocks = e->sm_count * 16;
+  DevBufs bufs;
   float *a = nullptr, *b = nullptr, *d = nullptr;
   double *d_noise = nullptr, *zbuf = nullptr, *d_w = nullptr;
   int *vbuf = nullptr, *d_coords = nullptr;
   unsigned long long* d_cnt = nullptr;
-  auto cleanup = [&]() {
-    cudaFree(a); cudaFree(b); cudaFree(d); cudaFree(d_w); cudaFree(d_noise); cudaFree(zbuf); cudaFree(vbuf);
-    cudaFree(d_coords); cudaFree(d_cnt);
-  };
   const int maxdim = std::max(cv.sz, cv.sy);
   const size_t maxlines = std::max((size_t)cv.sy * cv.sx, (size_t)cv.sz * cv.sx);
-  // adaptive threshold: gaussian sigma = 49/6, truncate 4 (seed.py:160-163)
-  const double sigma = 49.0 / 6.0;
-  const int radius = (int)(4.0 * sigma + 0.5);
-  std::vector<double> w(radius + 1);                 // w[0] = centre tap
-  {
-    double sum = 0;
-    for (int k = -radius; k <= radius; ++k) sum += std::exp(-0.5 / (sigma * sigma) * k * k);
-    for (int k = 0; k <= radius; ++k) w[k] = std::exp(-0.5 / (sigma * sigma) * k * k) / sum;
-  }
-  int rc = 0;
-  if (dev_alloc(&a, n, false) || dev_alloc(&b, n, false) || dev_alloc(&d, n, false) || dev_alloc(&d_w, w.size(), false) ||
-      dev_alloc(&vbuf, (size_t)maxdim * maxlines, false) || dev_alloc(&zbuf, 2 * (size_t)maxdim * maxlines, false) ||
-      dev_alloc(&d_coords, (size_t)cap * 3, false) || dev_alloc(&d_cnt, 2) || (noise && dev_alloc(&d_noise, n, false))) {
-    cleanup();
+  const std::vector<double> w = seed_gauss_weights();   // adaptive threshold
+  const int radius = (int)w.size() - 1;
+  if (bufs.get(&a, n) || bufs.get(&b, n) || bufs.get(&d, n) || bufs.get(&d_w, w.size()) ||
+      bufs.get(&vbuf, (size_t)maxdim * maxlines) || bufs.get(&zbuf, 2 * (size_t)maxdim * maxlines) ||
+      bufs.get(&d_coords, (size_t)cap * 3) || bufs.get(&d_cnt, 2, true) || (noise && bufs.get(&d_noise, n)))
     return 1;
-  }
   cudaStream_t st = cudaStreamPerThread;
-  bool ok = cudaMemcpyAsync(d_w, w.data(), w.size() * sizeof(double), cudaMemcpyHostToDevice, st) == cudaSuccess;
-  if (noise) ok = ok && cudaMemcpyAsync(d_noise, noise, n * sizeof(double), cudaMemcpyHostToDevice, st) == cudaSuccess;
+  CUDA_OK(cudaMemcpyAsync(d_w, w.data(), w.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+  if (noise) CUDA_OK(cudaMemcpyAsync(d_noise, noise, n * sizeof(double), cudaMemcpyHostToDevice, st));
   seedk::sobel_mag<<<blocks, 256, 0, st>>>(cv.image, cv.image_is_u8, cv.mean, cv.stddev, a, cv.sz, cv.sy, cv.sx);
   seedk::gauss_pass<<<blocks, 256, 0, st>>>(a, b, d_w, radius, 0, cv.sz, cv.sy, cv.sx);
   seedk::gauss_pass<<<blocks, 256, 0, st>>>(b, d, d_w, radius, 1, cv.sz, cv.sy, cv.sx);
@@ -1347,20 +1343,14 @@ int ffn_canvas_seed_peaks(FfnCanvas* c, const float voxel_size_zyx[3], const dou
   seedk::edt_line<<<blocks, 128, 0, st>>>(d, 0, cv.sz, cv.sy, cv.sx, voxel_size_zyx[0], vbuf, zbuf);
   seedk::finish_dt<<<blocks, 256, 0, st>>>(d, cv.seg, cv.mask, cv.seed_mask, n);
   seedk::peaks_kernel<<<blocks, 256, 0, st>>>(d, d_noise, cv.sz, cv.sy, cv.sx, 3, d_coords, (unsigned long long)cap, d_cnt + 1);
+  CUDA_OK(cudaGetLastError());
   unsigned long long counts[2] = {0, 0};
-  ok = ok && cudaGetLastError() == cudaSuccess;
-  ok = ok && cudaMemcpyAsync(counts, d_cnt, sizeof(counts), cudaMemcpyDeviceToHost, st) == cudaSuccess;
-  ok = ok && cudaStreamSynchronize(st) == cudaSuccess;
-  if (!ok) {
-    rc = fail(std::string("seed policy kernels failed: ") + cudaGetErrorString(cudaGetLastError()));
-  } else {
-    *n_out = counts[0] == 0 ? 0 : (int64_t)counts[1];   // everything is an edge: no seeds (seed.py:176-177)
-    const int64_t m = std::min<int64_t>(*n_out, cap);
-    if (m > 0 && cudaMemcpy(coords_out, d_coords, (size_t)m * 3 * sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess)
-      rc = fail("seed coordinate copy failed");
-  }
-  cleanup();
-  return rc;
+  CUDA_OK(cudaMemcpyAsync(counts, d_cnt, sizeof(counts), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+  *n_out = counts[0] == 0 ? 0 : (int64_t)counts[1];   // everything is an edge: no seeds (seed.py:176-177)
+  const int64_t m = std::min<int64_t>(*n_out, cap);
+  if (m > 0) CUDA_OK(cudaMemcpy(coords_out, d_coords, (size_t)m * 3 * sizeof(int), cudaMemcpyDeviceToHost));
+  return 0;
 }
 
 int ffn_canvas_seed_policy(FfnCanvas* c, const FfnSeedPolicyDesc* desc, const double* noise, int32_t* coords_out,
@@ -1377,47 +1367,31 @@ int ffn_canvas_seed_policy(FfnCanvas* c, const FfnSeedPolicyDesc* desc, const do
   const bool needs_edt = desc->kind != FFN_SEED_MAX_PEAKS;
   const size_t noise_n = is2d ? (size_t)cv.sy * cv.sx : n;
   const int blocks = e->sm_count * 16;
+  DevBufs bufs;
   float *a = nullptr, *b = nullptr, *d = nullptr;
   double *keys = nullptr, *m1 = nullptr, *m2 = nullptr, *d_noise = nullptr, *zbuf = nullptr, *d_w = nullptr;
   int *vbuf = nullptr, *d_coords = nullptr;
   unsigned long long* d_cnt = nullptr;   // [0] peaks, [1] / [2] ordered bits of the min / max key, [3] unused
   unsigned long long* d_smin = nullptr;  // 2-D threshold_abs=None: ordered bits of each z-slice's minimum key
-  auto cleanup = [&]() {
-    cudaFree(a); cudaFree(b); cudaFree(d); cudaFree(keys); cudaFree(m1); cudaFree(m2); cudaFree(d_noise); cudaFree(zbuf);
-    cudaFree(d_w); cudaFree(vbuf); cudaFree(d_coords); cudaFree(d_cnt); cudaFree(d_smin);
-  };
   const bool per_slice_min = is2d && desc->threshold_abs_is_min;
   // EDT scratch: 2-D sweeps only along y (lines (z, x)), 3-D also along z (lines (y, x))
   const int maxdim = is2d ? cv.sy : std::max(cv.sz, cv.sy);
   const size_t maxlines = is2d ? (size_t)cv.sz * cv.sx : std::max((size_t)cv.sy * cv.sx, (size_t)cv.sz * cv.sx);
-  // adaptive threshold of PolicyPeaks2d: gaussian sigma = 49/6, truncate 4 (seed.py:240-242)
-  const double sigma = 49.0 / 6.0;
-  const int radius = (int)(4.0 * sigma + 0.5);
-  std::vector<double> w(radius + 1);
-  {
-    double sum = 0;
-    for (int k = -radius; k <= radius; ++k) sum += std::exp(-0.5 / (sigma * sigma) * k * k);
-    for (int k = 0; k <= radius; ++k) w[k] = std::exp(-0.5 / (sigma * sigma) * k * k) / sum;
-  }
-  bool alloc_failed = dev_alloc(&d, n, false) || dev_alloc(&keys, n, false) || dev_alloc(&m1, n, false) ||
-                      dev_alloc(&m2, n, false) || dev_alloc(&d_coords, (size_t)cap * 3, false) || dev_alloc(&d_cnt, 4) ||
-                      (noise && dev_alloc(&d_noise, noise_n, false));
-  if (!alloc_failed && is2d)
-    alloc_failed = dev_alloc(&a, n, false) || dev_alloc(&b, n, false) || dev_alloc(&d_w, w.size(), false);
-  if (!alloc_failed && needs_edt)
-    alloc_failed = dev_alloc(&vbuf, (size_t)maxdim * maxlines, false) || dev_alloc(&zbuf, 2 * (size_t)maxdim * maxlines, false);
-  if (!alloc_failed && per_slice_min) alloc_failed = dev_alloc(&d_smin, (size_t)cv.sz, false);
-  if (alloc_failed) {
-    cleanup();
+  const std::vector<double> w = seed_gauss_weights();   // adaptive threshold of PolicyPeaks2d
+  const int radius = (int)w.size() - 1;
+  if (bufs.get(&d, n) || bufs.get(&keys, n) || bufs.get(&m1, n) || bufs.get(&m2, n) ||
+      bufs.get(&d_coords, (size_t)cap * 3) || bufs.get(&d_cnt, 4, true) || (noise && bufs.get(&d_noise, noise_n)) ||
+      (is2d && (bufs.get(&a, n) || bufs.get(&b, n) || bufs.get(&d_w, w.size()))) ||
+      (needs_edt && (bufs.get(&vbuf, (size_t)maxdim * maxlines) || bufs.get(&zbuf, 2 * (size_t)maxdim * maxlines))) ||
+      (per_slice_min && bufs.get(&d_smin, (size_t)cv.sz)))
     return 1;
-  }
   cudaStream_t st = cudaStreamPerThread;
   const unsigned long long cnt_init[3] = {0ull, ~0ull, 0ull};
-  bool ok = cudaMemcpyAsync(d_cnt, cnt_init, sizeof(cnt_init), cudaMemcpyHostToDevice, st) == cudaSuccess;
-  if (noise) ok = ok && cudaMemcpyAsync(d_noise, noise, noise_n * sizeof(double), cudaMemcpyHostToDevice, st) == cudaSuccess;
-  if (per_slice_min) ok = ok && cudaMemsetAsync(d_smin, 0xff, (size_t)cv.sz * sizeof(unsigned long long), st) == cudaSuccess;
+  CUDA_OK(cudaMemcpyAsync(d_cnt, cnt_init, sizeof(cnt_init), cudaMemcpyHostToDevice, st));
+  if (noise) CUDA_OK(cudaMemcpyAsync(d_noise, noise, noise_n * sizeof(double), cudaMemcpyHostToDevice, st));
+  if (per_slice_min) CUDA_OK(cudaMemsetAsync(d_smin, 0xff, (size_t)cv.sz * sizeof(unsigned long long), st));
   if (desc->kind == FFN_SEED_PEAKS_2D) {
-    ok = ok && cudaMemcpyAsync(d_w, w.data(), w.size() * sizeof(double), cudaMemcpyHostToDevice, st) == cudaSuccess;
+    CUDA_OK(cudaMemcpyAsync(d_w, w.data(), w.size() * sizeof(double), cudaMemcpyHostToDevice, st));
     seedk::sobel_mag2d<<<blocks, 256, 0, st>>>(cv.image, cv.image_is_u8, cv.mean, cv.stddev, a, cv.sz, cv.sy, cv.sx);
     seedk::gauss_pass<<<blocks, 256, 0, st>>>(a, b, d_w, radius, 1, cv.sz, cv.sy, cv.sx);
     seedk::gauss_pass<<<blocks, 256, 0, st>>>(b, d, d_w, radius, 2, cv.sz, cv.sy, cv.sx);
@@ -1444,21 +1418,14 @@ int ffn_canvas_seed_policy(FfnCanvas* c, const FfnSeedPolicyDesc* desc, const do
   seedk::peaks_select<<<blocks, 256, 0, st>>>(keys, rz > 0 ? m1 : m2, desc->threshold_abs, desc->threshold_abs_is_min,
                                               desc->use_threshold_rel, desc->threshold_rel, d_cnt + 1, d_smin, rz, r, r, cv.sz,
                                               cv.sy, cv.sx, d_coords, (unsigned long long)cap, d_cnt);
+  CUDA_OK(cudaGetLastError());
   unsigned long long count = 0;
-  ok = ok && cudaGetLastError() == cudaSuccess;
-  ok = ok && cudaMemcpyAsync(&count, d_cnt, sizeof(count), cudaMemcpyDeviceToHost, st) == cudaSuccess;
-  ok = ok && cudaStreamSynchronize(st) == cudaSuccess;
-  int rc = 0;
-  if (!ok) {
-    rc = fail(std::string("seed policy kernels failed: ") + cudaGetErrorString(cudaGetLastError()));
-  } else {
-    *n_out = (int64_t)count;
-    const int64_t m = std::min<int64_t>(*n_out, cap);
-    if (m > 0 && cudaMemcpy(coords_out, d_coords, (size_t)m * 3 * sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess)
-      rc = fail("seed coordinate copy failed");
-  }
-  cleanup();
-  return rc;
+  CUDA_OK(cudaMemcpyAsync(&count, d_cnt, sizeof(count), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+  *n_out = (int64_t)count;
+  const int64_t m = std::min<int64_t>(*n_out, cap);
+  if (m > 0) CUDA_OK(cudaMemcpy(coords_out, d_coords, (size_t)m * 3 * sizeof(int), cudaMemcpyDeviceToHost));
+  return 0;
 }
 
 int ffn_canvas_set_max_id(FfnCanvas* c, int64_t max_id) {
@@ -1529,44 +1496,48 @@ int ffn_decision_points(int device, const FfnDecisionPointDesc* desc, uint64_t* 
       return fail("subvolume box lies outside the volume");
   }
   cudaDeviceProp prop{};
-  if (check_device(device, &prop)) return 1;
-  CUDA_OK(cudaSetDevice(device));
+  if (use_device(device, &prop)) return 1;
   cudaStream_t st = cudaStreamPerThread;
   const int blocks = prop.multiProcessorCount * 16;
   DevBufs bufs;
 
   // Compaction: sorted unique ids and their counts; the kept ids (non-zero, not dust) in uint64 order.
-  u64 *d_lab = nullptr, *d_sorted = nullptr, *d_unique = nullptr, *d_kept = nullptr;
+  u64 *d_lab = nullptr, *d_sorted = nullptr, *d_unique = nullptr;
   unsigned* d_counts = nullptr;
   unsigned char* d_flags = nullptr;
   int* d_num = nullptr;   // [0] runs, [1] kept ids
-  char* d_temp = nullptr;
+  int nruns = (int)n;     // an upper bound until the run-length encoding has counted them
   if (bufs.get(&d_lab, n) || bufs.get(&d_sorted, n) || bufs.get(&d_unique, n) || bufs.get(&d_counts, n) ||
       bufs.get(&d_num, 2))
     return 1;
-  size_t tb_sort = 0, tb_rle = 0, tb_sel = 0;
-  CUDA_OK(cub::DeviceRadixSort::SortKeys(nullptr, tb_sort, d_lab, d_sorted, (int)n, 0, 64, st));
-  CUDA_OK(cub::DeviceRunLengthEncode::Encode(nullptr, tb_rle, d_sorted, d_unique, d_counts, d_num, (int)n, st));
-  CUDA_OK(cub::DeviceSelect::Flagged(nullptr, tb_sel, d_unique, d_flags, d_sorted, d_num + 1, (int)n, st));
-  if (bufs.get(&d_temp, std::max(tb_sort, std::max(tb_rle, tb_sel)))) return 1;
+  u64* const d_kept = d_sorted;   // the sorted copy is no longer needed once the runs are encoded
+  auto sort = [&](void* t, size_t& b) {
+    return cub::DeviceRadixSort::SortKeys(t, b, d_lab, d_sorted, (int)n, 0, 64, st);
+  };
+  auto rle = [&](void* t, size_t& b) {
+    return cub::DeviceRunLengthEncode::Encode(t, b, d_sorted, d_unique, d_counts, d_num, (int)n, st);
+  };
+  auto select = [&](void* t, size_t& b) {
+    return cub::DeviceSelect::Flagged(t, b, d_unique, d_flags, d_kept, d_num + 1, nruns, st);
+  };
+  CubTemp temp;
+  if (temp.alloc(bufs, sort, rle, select)) return 1;
   CUDA_OK(cudaMemcpyAsync(d_lab, labels, n * sizeof(u64), cudaMemcpyHostToDevice, st));
-  CUDA_OK(cub::DeviceRadixSort::SortKeys(d_temp, tb_sort, d_lab, d_sorted, (int)n, 0, 64, st));
-  CUDA_OK(cub::DeviceRunLengthEncode::Encode(d_temp, tb_rle, d_sorted, d_unique, d_counts, d_num, (int)n, st));
-  int nruns = 0;
+  CUDA_OK(temp.run(sort));
+  CUDA_OK(temp.run(rle));
   u64 first_id = 0;
   CUDA_OK(cudaMemcpyAsync(&nruns, d_num, sizeof(int), cudaMemcpyDeviceToHost, st));
   CUDA_OK(cudaMemcpyAsync(&first_id, d_unique, sizeof(u64), cudaMemcpyDeviceToHost, st));
   CUDA_OK(cudaStreamSynchronize(st));
   if (bufs.get(&d_flags, nruns)) return 1;
   dpk::flag_kept<<<blocks, 256, 0, st>>>(d_unique, d_counts, nruns, desc->dust_threshold, d_flags);
-  d_kept = d_sorted;   // the sorted copy is no longer needed
-  CUDA_OK(cub::DeviceSelect::Flagged(d_temp, tb_sel, d_unique, d_flags, d_kept, d_num + 1, nruns, st));
+  CUDA_OK(temp.run(select));
   int nkept = 0;
   CUDA_OK(cudaMemcpyAsync(&nkept, d_num + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
   CUDA_OK(cudaStreamSynchronize(st));
   bufs.release(d_unique);
   bufs.release(d_counts);
-  bufs.release(d_temp);
+  bufs.release(temp.p);
   bufs.release(d_flags);
   const bool dust_cleared = nkept < nruns - (first_id == 0 ? 1 : 0);
 
@@ -1688,8 +1659,7 @@ int ffn_reseg_eval(int device, const FfnResegEvalDesc* desc, const uint64_t* lab
   *n_overlaps = 0;
   if (nitems == 0) return 0;
   cudaDeviceProp prop{};
-  if (check_device(device, &prop)) return 1;
-  CUDA_OK(cudaSetDevice(device));
+  if (use_device(device, &prop)) return 1;
   cudaStream_t st = cudaStreamPerThread;
   const int blocks = prop.multiProcessorCount * 16;
   // Items (grid y) x blocks per box (grid x): about 16 resident blocks per SM over the whole batch.
@@ -1764,40 +1734,43 @@ int ffn_reseg_eval(int device, const FfnResegEvalDesc* desc, const uint64_t* lab
   int ibits = 1;
   while ((1ll << ibits) < nitems) ++ibits;
   const int ni = (int)n;
+  int nruns = ni;   // an upper bound until the runs are counted: at most one row per voxel
   u64* d_lab2 = nullptr;
   unsigned *d_vals = nullptr, *d_vals2 = nullptr, *d_scan = nullptr;
   unsigned char* d_head = nullptr;
   int *d_heads = nullptr, *d_num = nullptr;
-  char* d_temp = nullptr;
+  FfnResegOverlap *d_all = nullptr, *d_kept = nullptr;
   if (bufs.get(&d_lab2, n) || bufs.get(&d_vals, n) || bufs.get(&d_vals2, n) || bufs.get(&d_scan, n) ||
       bufs.get(&d_head, n) || bufs.get(&d_heads, n) || bufs.get(&d_num, 2))
     return 1;
   rsk::endpoint_prepare<<<item_grid, 256, 0, st>>>(d_lab, d_probs, d_ids, d_table, nitems, nbox, d_vals, d_counts);
-  FfnResegOverlap* d_rows = nullptr;   // only sized here: at most one row per voxel
-  size_t tb[5] = {0, 0, 0, 0, 0};
-  CUDA_OK(cub::DeviceRadixSort::SortPairs(nullptr, tb[0], d_lab, d_lab2, d_vals, d_vals2, ni, 0, 64, st));
-  CUDA_OK(cub::DeviceRadixSort::SortPairs(nullptr, tb[1], d_vals2, d_vals, d_lab2, d_lab, ni, 1, 1 + ibits, st));
-  CUDA_OK(cub::DeviceSelect::Flagged(nullptr, tb[2], cub::CountingInputIterator<int>(0), d_head, d_heads, d_num, ni, st));
-  CUDA_OK(cub::DeviceScan::InclusiveSum(nullptr, tb[3], d_vals2, d_scan, ni, st));
-  CUDA_OK(cub::DeviceSelect::If(nullptr, tb[4], d_rows, d_rows, d_num + 1, ni, rsk::Overlapping(), st));
-  if (bufs.get(&d_temp, *std::max_element(tb, tb + 5))) return 1;
-  CUDA_OK(cub::DeviceRadixSort::SortPairs(d_temp, tb[0], d_lab, d_lab2, d_vals, d_vals2, ni, 0, 64, st));
-  CUDA_OK(cub::DeviceRadixSort::SortPairs(d_temp, tb[1], d_vals2, d_vals, d_lab2, d_lab, ni, 1, 1 + ibits, st));
+  auto sort_label = [&](void* t, size_t& b) {
+    return cub::DeviceRadixSort::SortPairs(t, b, d_lab, d_lab2, d_vals, d_vals2, ni, 0, 64, st);
+  };
+  auto sort_item = [&](void* t, size_t& b) {
+    return cub::DeviceRadixSort::SortPairs(t, b, d_vals2, d_vals, d_lab2, d_lab, ni, 1, 1 + ibits, st);
+  };
+  auto select_heads = [&](void* t, size_t& b) {
+    return cub::DeviceSelect::Flagged(t, b, cub::CountingInputIterator<int>(0), d_head, d_heads, d_num, ni, st);
+  };
+  auto scan = [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, d_vals2, d_scan, ni, st); };
+  auto select_rows = [&](void* t, size_t& b) {
+    return cub::DeviceSelect::If(t, b, d_all, d_kept, d_num + 1, nruns, rsk::Overlapping(), st);
+  };
+  CubTemp temp;
+  if (temp.alloc(bufs, sort_label, sort_item, select_heads, scan, select_rows)) return 1;
+  CUDA_OK(temp.run(sort_label));
+  CUDA_OK(temp.run(sort_item));
   // Sorted by (item, label): d_vals = item << 1 | mask, d_lab = label.
   rsk::run_heads<<<blocks, 256, 0, st>>>(d_vals, d_lab, ni, d_head, d_vals2);
-  CUDA_OK(cub::DeviceSelect::Flagged(d_temp, tb[2], cub::CountingInputIterator<int>(0), d_head, d_heads, d_num, ni, st));
-  CUDA_OK(cub::DeviceScan::InclusiveSum(d_temp, tb[3], d_vals2, d_scan, ni, st));
-  int nruns = 0;
+  CUDA_OK(temp.run(select_heads));
+  CUDA_OK(temp.run(scan));
   CUDA_OK(cudaMemcpyAsync(&nruns, d_num, sizeof(int), cudaMemcpyDeviceToHost, st));
   CUDA_OK(cudaMemcpyAsync(counts.data(), d_counts, counts.size() * sizeof(u64), cudaMemcpyDeviceToHost, st));
   CUDA_OK(cudaStreamSynchronize(st));
-  FfnResegOverlap *d_all = nullptr, *d_kept = nullptr;
   if (bufs.get(&d_all, nruns) || bufs.get(&d_kept, nruns)) return 1;
   rsk::run_rows<<<blocks, 256, 0, st>>>(d_heads, nruns, ni, d_vals, d_lab, d_scan, d_all);
-  size_t tb_keep = 0;
-  CUDA_OK(cub::DeviceSelect::If(nullptr, tb_keep, d_all, d_kept, d_num + 1, nruns, rsk::Overlapping(), st));
-  if (tb_keep > tb[4]) return fail("overlap selection needs more temporary storage than planned");
-  CUDA_OK(cub::DeviceSelect::If(d_temp, tb_keep, d_all, d_kept, d_num + 1, nruns, rsk::Overlapping(), st));
+  CUDA_OK(temp.run(select_rows));
   CUDA_OK(cudaGetLastError());
   int nkept = 0;
   CUDA_OK(cudaMemcpyAsync(&nkept, d_num + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -1827,33 +1800,48 @@ int ffn_split_intersection(int device, int64_t n, uint64_t* a, const uint64_t* b
   if (n >= (1ll << 31)) return fail("split consensus supports volumes of fewer than 2^31 voxels");
   if (n == 0) return 0;
   cudaDeviceProp prop{};
-  if (check_device(device, &prop)) return 1;
-  CUDA_OK(cudaSetDevice(device));
+  if (use_device(device, &prop)) return 1;
   cudaStream_t st = cudaStreamPerThread;
   const int blocks = prop.multiProcessorCount * 16;
   const int ni = (int)n;
+  int np = ni;   // an upper bound until the (a, b) pairs are counted
   DevBufs bufs;
 
   u64 *d_a = nullptr, *d_b = nullptr, *d_tmp = nullptr, *d_max = nullptr;
   int* d_num = nullptr;
-  char* d_temp = nullptr;
   if (bufs.get(&d_a, n) || bufs.get(&d_b, n) || bufs.get(&d_tmp, n) || bufs.get(&d_max, 2) || bufs.get(&d_num, 2))
     return 1;
-  // Temporary storage for every CUB call below, sized for n items (no later call has more).
-  size_t tb[7] = {0, 0, 0, 0, 0, 0, 0};
-  CUDA_OK(cub::DeviceReduce::Max(nullptr, tb[0], d_a, d_max, ni, st));
-  CUDA_OK(cub::DeviceRadixSort::SortKeys(nullptr, tb[1], d_a, d_tmp, ni, 0, 64, st));
-  CUDA_OK(cub::DeviceSelect::Unique(nullptr, tb[2], d_tmp, d_a, d_num, ni, st));
-  CUDA_OK(cub::DeviceRunLengthEncode::Encode(nullptr, tb[3], d_tmp, d_a, (int*)d_b, d_num, ni, st));
-  CUDA_OK(cub::DeviceRadixSort::SortPairs(nullptr, tb[4], d_tmp, d_a, (int*)d_b, (int*)d_b, ni, 0, 64, st));
-  CUDA_OK(cub::DeviceReduce::ReduceByKey(nullptr, tb[5], (unsigned*)d_a, (unsigned*)d_b, d_tmp, d_a, d_num,
-                                         MaxU64(), ni, st));
-  CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, tb[6], (int*)d_a, (int*)d_b, ni, st));
-  if (bufs.get(&d_temp, *std::max_element(tb, tb + 7))) return 1;
+  u64 *d_pairs = nullptr, *d_sw = nullptr, *d_sw2 = nullptr, *d_pack = nullptr, *d_best = nullptr, *d_lab = nullptr;
+  int *d_counts = nullptr, *d_idx = nullptr, *d_idx2 = nullptr, *d_flags = nullptr, *d_rank = nullptr;
+  unsigned *d_aof = nullptr, *d_ured = nullptr;
+  unsigned char* d_partner = nullptr;
+  // The CUB calls (max_of, sort_keys and unique run on several arrays), sized for n items: no later call has more.
+  auto max_of = [&](u64* in, u64* out) {
+    return [=](void* t, size_t& b) { return cub::DeviceReduce::Max(t, b, in, out, ni, st); };
+  };
+  auto sort_keys = [&](u64* in, u64* out) {
+    return [=](void* t, size_t& b) { return cub::DeviceRadixSort::SortKeys(t, b, in, out, ni, 0, 64, st); };
+  };
+  auto unique = [&](u64* out) {
+    return [=](void* t, size_t& b) { return cub::DeviceSelect::Unique(t, b, d_tmp, out, d_num, ni, st); };
+  };
+  auto rle = [&](void* t, size_t& b) {
+    return cub::DeviceRunLengthEncode::Encode(t, b, d_b, d_pairs, d_counts, d_num, ni, st);
+  };
+  auto sort_pairs = [&](void* t, size_t& b) {
+    return cub::DeviceRadixSort::SortPairs(t, b, d_sw, d_sw2, d_idx, d_idx2, np, 0, 64, st);
+  };
+  auto reduce_best = [&](void* t, size_t& b) {
+    return cub::DeviceReduce::ReduceByKey(t, b, d_aof, d_ured, d_pack, d_best, d_num + 1, MaxU64(), np, st);
+  };
+  auto scan = [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_flags, d_rank, np, st); };
+  CubTemp temp;
+  if (temp.alloc(bufs, max_of(d_a, d_max), sort_keys(d_a, d_tmp), unique(d_a), rle, sort_pairs, reduce_best, scan))
+    return 1;
   CUDA_OK(cudaMemcpyAsync(d_a, a, n * sizeof(u64), cudaMemcpyHostToDevice, st));
   CUDA_OK(cudaMemcpyAsync(d_b, b, n * sizeof(u64), cudaMemcpyHostToDevice, st));
-  CUDA_OK(cub::DeviceReduce::Max(d_temp, tb[0], d_a, d_max, ni, st));
-  CUDA_OK(cub::DeviceReduce::Max(d_temp, tb[0], d_b, d_max + 1, ni, st));
+  CUDA_OK(temp.run(max_of(d_a, d_max)));
+  CUDA_OK(temp.run(max_of(d_b, d_max + 1)));
   u64 maxes[2] = {0, 0};
   CUDA_OK(cudaMemcpyAsync(maxes, d_max, sizeof(maxes), cudaMemcpyDeviceToHost, st));
   CUDA_OK(cudaStreamSynchronize(st));
@@ -1865,9 +1853,9 @@ int ffn_split_intersection(int device, int64_t n, uint64_t* a, const uint64_t* b
   unsigned shift[2] = {0, 0};
   for (int k = 0; k < 2; ++k) {
     if (maxes[k] <= 0xffffffffull) continue;
-    CUDA_OK(cub::DeviceRadixSort::SortKeys(d_temp, tb[1], k ? d_b : d_a, d_tmp, ni, 0, 64, st));
+    CUDA_OK(temp.run(sort_keys(k ? d_b : d_a, d_tmp)));
     if (bufs.get(&uniq[k], n)) return 1;
-    CUDA_OK(cub::DeviceSelect::Unique(d_temp, tb[2], d_tmp, uniq[k], d_num, ni, st));
+    CUDA_OK(temp.run(unique(uniq[k])));
     u64 first = 0;
     CUDA_OK(cudaMemcpyAsync(&nuniq[k], d_num, sizeof(int), cudaMemcpyDeviceToHost, st));
     CUDA_OK(cudaMemcpyAsync(&first, uniq[k], sizeof(u64), cudaMemcpyDeviceToHost, st));
@@ -1880,29 +1868,22 @@ int ffn_split_intersection(int device, int64_t n, uint64_t* a, const uint64_t* b
                                           shift[1], d_tmp);
   CUDA_OK(cudaGetLastError());
   if (uniq[1]) bufs.release(uniq[1]);
-  CUDA_OK(cub::DeviceRadixSort::SortKeys(d_temp, tb[1], d_tmp, d_b, ni, 0, 64, st));
-  u64* d_pairs = nullptr;
-  int* d_counts = nullptr;
+  CUDA_OK(temp.run(sort_keys(d_tmp, d_b)));
   if (bufs.get(&d_pairs, n) || bufs.get(&d_counts, n)) return 1;
-  CUDA_OK(cub::DeviceRunLengthEncode::Encode(d_temp, tb[3], d_b, d_pairs, d_counts, d_num, ni, st));
-  int np = 0;
+  CUDA_OK(temp.run(rle));
   CUDA_OK(cudaMemcpyAsync(&np, d_num, sizeof(int), cudaMemcpyDeviceToHost, st));
   CUDA_OK(cudaStreamSynchronize(st));
   bufs.release(d_b);
 
   // Largest overlap per a: the pairs regrouped by a (a-major sort), then a maximum of count << 32 | ~b per a.
-  u64 *d_sw = nullptr, *d_sw2 = nullptr, *d_pack = nullptr, *d_best = nullptr, *d_lab = nullptr;
-  int *d_idx = nullptr, *d_idx2 = nullptr, *d_flags = nullptr, *d_rank = nullptr;
-  unsigned *d_aof = nullptr, *d_ured = nullptr;
-  unsigned char* d_partner = nullptr;
   if (bufs.get(&d_sw, np) || bufs.get(&d_sw2, np) || bufs.get(&d_pack, np) || bufs.get(&d_best, np) ||
       bufs.get(&d_lab, np) || bufs.get(&d_idx, np) || bufs.get(&d_idx2, np) || bufs.get(&d_flags, np) ||
       bufs.get(&d_rank, np) || bufs.get(&d_aof, np) || bufs.get(&d_ured, np) || bufs.get(&d_partner, np))
     return 1;
   csk::regroup<<<blocks, 256, 0, st>>>(d_pairs, np, d_sw, d_idx);
-  CUDA_OK(cub::DeviceRadixSort::SortPairs(d_temp, tb[4], d_sw, d_sw2, d_idx, d_idx2, np, 0, 64, st));
+  CUDA_OK(temp.run(sort_pairs));
   csk::partner_pack<<<blocks, 256, 0, st>>>(d_sw2, d_idx2, d_counts, np, d_aof, d_pack);
-  CUDA_OK(cub::DeviceReduce::ReduceByKey(d_temp, tb[5], d_aof, d_ured, d_pack, d_best, d_num + 1, MaxU64(), np, st));
+  CUDA_OK(temp.run(reduce_best));
   int nu = 0;
   CUDA_OK(cudaMemcpyAsync(&nu, d_num + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
   CUDA_OK(cudaStreamSynchronize(st));
@@ -1910,7 +1891,7 @@ int ffn_split_intersection(int device, int64_t n, uint64_t* a, const uint64_t* b
 
   // New ids in key order, then the output id of every pair.
   csk::pair_flags<<<blocks, 256, 0, st>>>(d_pairs, d_counts, d_partner, np, (long long)min_size, d_flags);
-  CUDA_OK(cub::DeviceScan::ExclusiveSum(d_temp, tb[6], d_flags, d_rank, np, st));
+  CUDA_OK(temp.run(scan));
   int last[2] = {0, 0};
   CUDA_OK(cudaMemcpyAsync(&last[0], d_flags + np - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
   CUDA_OK(cudaMemcpyAsync(&last[1], d_rank + np - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -1951,8 +1932,7 @@ int ffn_compute_partitions(int device, const FfnPartitionDesc* desc, uint64_t* l
   if (desc->n_labels_out) *desc->n_labels_out = 0;
   if (n == 0) return 0;
   cudaDeviceProp prop{};
-  if (check_device(device, &prop)) return 1;
-  CUDA_OK(cudaSetDevice(device));
+  if (use_device(device, &prop)) return 1;
   cudaStream_t st = cudaStreamPerThread;
   const int blocks = prop.multiProcessorCount * 16;
   const int ni = (int)n;
@@ -1962,17 +1942,18 @@ int ffn_compute_partitions(int device, const FfnPartitionDesc* desc, uint64_t* l
   u64 *d_lab = nullptr, *d_sorted = nullptr, *d_unique = nullptr;
   unsigned* d_cnt = nullptr;
   int* d_num = nullptr;
-  char* d_temp = nullptr;
   if (bufs.get(&d_lab, n) || bufs.get(&d_sorted, n) || bufs.get(&d_unique, n) || bufs.get(&d_cnt, n) ||
       bufs.get(&d_num, 1))
     return 1;
-  size_t tb_sort = 0, tb_rle = 0;
-  CUDA_OK(cub::DeviceRadixSort::SortKeys(nullptr, tb_sort, d_lab, d_sorted, ni, 0, 64, st));
-  CUDA_OK(cub::DeviceRunLengthEncode::Encode(nullptr, tb_rle, d_sorted, d_unique, d_cnt, d_num, ni, st));
-  if (bufs.get(&d_temp, std::max(tb_sort, tb_rle))) return 1;
+  auto sort = [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortKeys(t, b, d_lab, d_sorted, ni, 0, 64, st); };
+  auto rle = [&](void* t, size_t& b) {
+    return cub::DeviceRunLengthEncode::Encode(t, b, d_sorted, d_unique, d_cnt, d_num, ni, st);
+  };
+  CubTemp temp;
+  if (temp.alloc(bufs, sort, rle)) return 1;
   CUDA_OK(cudaMemcpyAsync(d_lab, labels, n * sizeof(u64), cudaMemcpyHostToDevice, st));
-  CUDA_OK(cub::DeviceRadixSort::SortKeys(d_temp, tb_sort, d_lab, d_sorted, ni, 0, 64, st));
-  CUDA_OK(cub::DeviceRunLengthEncode::Encode(d_temp, tb_rle, d_sorted, d_unique, d_cnt, d_num, ni, st));
+  CUDA_OK(temp.run(sort));
+  CUDA_OK(temp.run(rle));
   int nruns = 0;
   CUDA_OK(cudaMemcpyAsync(&nruns, d_num, sizeof(int), cudaMemcpyDeviceToHost, st));
   CUDA_OK(cudaStreamSynchronize(st));
@@ -1983,7 +1964,7 @@ int ffn_compute_partitions(int device, const FfnPartitionDesc* desc, uint64_t* l
   CUDA_OK(cudaStreamSynchronize(st));
   bufs.release(d_sorted);
   bufs.release(d_cnt);
-  bufs.release(d_temp);
+  bufs.release(temp.p);
 
   // Run codes: dust (cleared), skipped (0, or outside the whitelist) or the compact id, in uint64 id order.
   std::vector<u64> white(desc->whitelist, desc->whitelist + desc->n_whitelist);
@@ -2166,8 +2147,7 @@ int ffn_partition_rows(int device, const FfnPartitionRowsDesc* desc, const uint8
   std::fill(counts, counts + 256, (int64_t)0);
   if (ncrop == 0) return 0;
   cudaDeviceProp prop{};
-  if (check_device(device, &prop)) return 1;
-  CUDA_OK(cudaSetDevice(device));
+  if (use_device(device, &prop)) return 1;
   cudaStream_t st = cudaStreamPerThread;
   const int ntiles = (int)((ncrop + cok::kTile - 1) / cok::kTile);
   const size_t nhist = (size_t)256 * ntiles;
@@ -2176,21 +2156,22 @@ int ffn_partition_rows(int device, const FfnPartitionRowsDesc* desc, const uint8
   int *d_hist = nullptr, *d_base = nullptr;
   unsigned long long* d_counts = nullptr;
   longlong2* d_rows = nullptr;
-  char* d_temp = nullptr;
-  size_t tb = 0;
-  CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, tb, d_hist, d_base, (int64_t)nhist, st));
+  auto scan = [&](void* t, size_t& b) {
+    return cub::DeviceScan::ExclusiveSum(t, b, d_hist, d_base, (int64_t)nhist, st);
+  };
+  CubTemp temp;
   if (bufs.get(&d_vol, nvol) || bufs.get(&d_hist, nhist) || bufs.get(&d_base, nhist) || bufs.get(&d_counts, 256) ||
-      bufs.get(&d_temp, tb))
+      temp.alloc(bufs, scan))
     return 1;
   CUDA_OK(cudaMemcpyAsync(d_vol, volume, nvol, cudaMemcpyHostToDevice, st));
   CUDA_OK(cudaMemsetAsync(d_counts, 0, 256 * sizeof(unsigned long long), st));
   cok::bucket_hist<<<ntiles, cok::kThreads, 0, st>>>(d_vol, c, ntiles, d_hist, d_counts);
   CUDA_OK(cudaGetLastError());
-  CUDA_OK(cub::DeviceScan::ExclusiveSum(d_temp, tb, d_hist, d_base, (int64_t)nhist, st));
+  CUDA_OK(temp.run(scan));
   CUDA_OK(cudaMemcpyAsync(counts, d_counts, 256 * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
   CUDA_OK(cudaStreamSynchronize(st));
   bufs.release(d_hist);
-  bufs.release(d_temp);
+  bufs.release(temp.p);
   const long long kept = ncrop - counts[cok::kIgnore];
   if (bufs.get(&d_rows, kept)) return 1;
   cok::bucket_scatter<<<ntiles, cok::kThreads, 0, st>>>(d_vol, c, ntiles, d_base, desc->volume_index, d_rows);
@@ -2226,8 +2207,7 @@ int ffn_coordinate_records(int device, const FfnCoordinateDesc* desc, const int6
   *out_bytes = 0;
   if (n_rows == 0) return 0;
   cudaDeviceProp prop{};
-  if (check_device(device, &prop)) return 1;
-  CUDA_OK(cudaSetDevice(device));
+  if (use_device(device, &prop)) return 1;
   cudaStream_t st = cudaStreamPerThread;
   const long long nblocks = (n_rows + cok::kThreads - 1) / cok::kThreads;
   DevBufs bufs;
@@ -2236,11 +2216,12 @@ int ffn_coordinate_records(int device, const FfnCoordinateDesc* desc, const int6
   unsigned char *d_names = nullptr, *d_out = nullptr;
   cok::u64 *d_sums = nullptr, *d_offs = nullptr;
   int* d_bad = nullptr;
-  char* d_temp = nullptr;
-  size_t tb = 0;
-  CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, tb, d_sums, d_offs, (int64_t)nblocks + 1, st));
+  auto scan = [&](void* t, size_t& b) {
+    return cub::DeviceScan::ExclusiveSum(t, b, d_sums, d_offs, (int64_t)nblocks + 1, st);
+  };
+  CubTemp temp;
   if (bufs.get(&d_rows, n_rows) || bufs.get(&d_vols, vols.size()) || bufs.get(&d_names, desc->names_bytes) ||
-      bufs.get(&d_sums, nblocks + 1) || bufs.get(&d_offs, nblocks + 1) || bufs.get(&d_bad, 1) || bufs.get(&d_temp, tb))
+      bufs.get(&d_sums, nblocks + 1) || bufs.get(&d_offs, nblocks + 1) || bufs.get(&d_bad, 1) || temp.alloc(bufs, scan))
     return 1;
   CUDA_OK(cudaMemcpyAsync(d_rows, rows, n_rows * sizeof(longlong2), cudaMemcpyHostToDevice, st));
   if (!vols.empty())
@@ -2251,7 +2232,7 @@ int ffn_coordinate_records(int device, const FfnCoordinateDesc* desc, const int6
   CUDA_OK(cudaMemsetAsync(d_bad, 0, sizeof(int), st));
   cok::record_sums<<<(unsigned)nblocks, cok::kThreads, 0, st>>>(d_rows, n_rows, d_vols, desc->n_volumes, d_sums, d_bad);
   CUDA_OK(cudaGetLastError());
-  CUDA_OK(cub::DeviceScan::ExclusiveSum(d_temp, tb, d_sums, d_offs, (int64_t)nblocks + 1, st));
+  CUDA_OK(temp.run(scan));
   cok::u64 total = 0;
   int bad = 0;
   CUDA_OK(cudaMemcpyAsync(&total, d_offs + nblocks, sizeof(total), cudaMemcpyDeviceToHost, st));
