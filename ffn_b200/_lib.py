@@ -35,7 +35,7 @@ EXPORTS = [
     'ffn_canvas_policy_state_size', 'ffn_canvas_policy_state_get', 'ffn_canvas_policy_state_set',
     'ffn_canvas_set_resume', 'ffn_canvas_trace', 'ffn_canvas_seed_peaks', 'ffn_canvas_seed_policy', 'ffn_canvas_set_max_id', 'ffn_canvas_get_counters', 'ffn_canvas_spec_stats', 'ffn_canvas_sched_stats', 'ffn_canvas_device_ptr',
     'ffn_canvas_add_id_offset', 'ffn_decision_points', 'ffn_reseg_eval', 'ffn_split_intersection', 'ffn_compute_partitions',
-    'ffn_partition_rows', 'ffn_coordinate_records', 'ffn_selftest_wgmma',
+    'ffn_partition_rows', 'ffn_coordinate_records', 'ffn_clean_up', 'ffn_selftest_wgmma',
 ]
 
 
@@ -93,6 +93,10 @@ class PartitionDesc(C.Structure):
 class PartitionRowsDesc(C.Structure):
   _fields_ = [('shape_zyx', C.c_int32 * 3), ('crop_start_zyx', C.c_int32 * 3), ('crop_shape_zyx', C.c_int32 * 3),
               ('reserved', C.c_int32), ('volume_index', C.c_int64)]
+
+
+class CleanUpDesc(C.Structure):
+  _fields_ = [('shape_zyx', C.c_int32 * 3), ('connectivity', C.c_int32), ('min_size', C.c_int64)]
 
 
 class CoordinateVolume(C.Structure):
@@ -199,6 +203,7 @@ def load() -> C.CDLL:
   lib.ffn_partition_rows.argtypes = [C.c_int, C.POINTER(PartitionRowsDesc), p, p, p]
   lib.ffn_coordinate_records.argtypes = [C.c_int, C.POINTER(CoordinateDesc), p, C.c_int64, p, C.c_int64,
                                          C.POINTER(C.c_int64)]
+  lib.ffn_clean_up.argtypes = [C.c_int, C.POINTER(CleanUpDesc), p, p, p, p, C.c_int64, C.POINTER(C.c_int64)]
   lib.ffn_selftest_wgmma.argtypes = [C.c_int, C.POINTER(C.c_double), C.c_int]
   for name in EXPORTS:
     if name not in ('ffn_last_error', 'ffn_engine_destroy', 'ffn_canvas_destroy'):

@@ -428,6 +428,23 @@ typedef struct {
 int ffn_coordinate_records(int device, const FfnCoordinateDesc* desc, const int64_t* rows, int64_t n_rows,
                            uint8_t* out, int64_t out_capacity, int64_t* out_bytes);
 
+/* ---- connected components: clean_up / clean_up_and_count (ffn/inference/segmentation.py:89-178) ------------------
+ * A component is a maximal set of voxels of one non-zero id connected under 6- (1), 18- (2) or 26-connectivity (3).
+ * Components are numbered 1, 2, ... in C order of their first voxel; 0 stays 0.  Then every component with fewer than
+ * min_size voxels becomes 0 (its number stays unused). */
+typedef struct {
+  int32_t shape_zyx[3];
+  int32_t connectivity;   /* 1, 2 or 3 */
+  int64_t min_size;       /* <= 0: no size filter */
+} FfnCleanUpDesc;
+/* labels: host uint64 [z][y][x], rewritten in place with the component numbers.  Table (ids, orig_ids, counts, each
+ * optional; all NULL with cap = 0 when no table is wanted): one row per output id in ascending order, 0 first when the
+ * output has a 0: the id, the input id at the id's first voxel in the output, and its voxel count.  *n_ids: the rows.
+ * When a table is wanted and *n_ids > cap, nothing is written, labels included: call again with cap = *n_ids.  Fails
+ * for 2^31 or more voxels, a negative extent or a connectivity other than 1, 2, 3. */
+int ffn_clean_up(int device, const FfnCleanUpDesc* desc, uint64_t* labels, uint64_t* ids, uint64_t* orig_ids,
+                 int64_t* counts, int64_t cap, int64_t* n_ids);
+
 /* Known-answer test of the wgmma descriptors (worst absolute error of each case in out[]; see
  * ffn_b200/csrc/selftest.cuh).  Used by tests, not by the product path. */
 int ffn_selftest_wgmma(int device, double* out, int n_out);
