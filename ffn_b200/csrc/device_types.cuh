@@ -34,6 +34,16 @@ constexpr int kSplitShift = 10;   // FFN_COMPUTE_FP16X2_TC: weights are split as
 constexpr int kMaxTilesPerCta = 0xFFFF / kTileOut;   // the per-CTA step counts are packed into 16 bits (publish_counts)
 static_assert(kMaxChains >= 1 && kMaxChains <= 5, "chains");
 
+// Named barriers of the flood kernel (0: __syncthreads, 4: grid_barrier's release of the CTA, 5: publish_counts of the
+// eight consumer warps).  A consumer warpgroup orders its own neighbour exchange with kBarXchg0 + warpgroup (128
+// threads); warps 3 and 4, on either side of the seam between the warpgroups' accumulator rows, hand over rows 63 and
+// 64 through kBarSeamUp (warp 3 -> warp 4) and kBarSeamDn (warp 4 -> warp 3), 64 threads each.  The fp16 path lets
+// the warpgroups issue their MMAs in turn: kBarOrder0 + w (256 threads) opens warpgroup w's turn.
+constexpr int kBarXchg0 = 1;      // and 2
+constexpr int kBarSeamUp = 6;
+constexpr int kBarSeamDn = 7;
+constexpr int kBarOrder0 = 8;     // and 9
+
 // Field-of-view geometry in the "row" space the kernels work in.
 //
 // A FoV voxel (z, y, x) lives at row  r = z * pp + y * xp + x  with xp = fx and pp = (fy + 1) * xp:

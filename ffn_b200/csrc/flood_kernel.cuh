@@ -520,7 +520,17 @@ __device__ __forceinline__ int tc_epilogue(Ctx& c, int k, int layer, int tile, c
 #pragma unroll
     for (int i = 0; i < 4; ++i) x2[((c.warp * 2 + 1) * 4 + i) * 4 + t] = make_float2(ACC(2, 0, 2 * i), ACC(2, 0, 2 * i + 1));
   }
-  asm volatile("bar.sync 3, 256;" ::: "memory");
+  // The two warpgroups meet only at the seam between accumulator rows 63 (warp 3) and 64 (warp 4); inside a warpgroup
+  // one 128-thread barrier orders the exchange.  Warp 4 syncs on warp 3's row-63 values BEFORE it announces its own
+  // row-64 values, and warp 3 waits for those only after that: so neither warp can arrive at a seam barrier twice
+  // before the other has consumed the first arrival, whatever the skew between the warpgroups.
+  if (c.warp == 3) asm volatile("bar.arrive %0, 64;" ::"n"(kBarSeamUp) : "memory");   // D[63][dx=-1] stored
+  if (c.warp == 4) {
+    asm volatile("bar.sync %0, 64;" ::"n"(kBarSeamUp) : "memory");
+    asm volatile("bar.arrive %0, 64;" ::"n"(kBarSeamDn) : "memory");                    // D[64][dx=+1] stored
+  }
+  if (c.warp < 4) asm volatile("bar.sync %0, 128;" ::"n"(kBarXchg0) : "memory");
+  else asm volatile("bar.sync %0, 128;" ::"n"(kBarXchg0 + 1) : "memory");
   // up[h][q] = D[m-1][dx=-1], dn[h][q] = D[m+1][dx=+1] for the rows m = m0 + 8 h
   const int src_up = (c.lane + 28) & 31, src_dn = (c.lane + 4) & 31;
   float up[2][8], dn[2][8];
@@ -541,14 +551,6 @@ __device__ __forceinline__ int tc_epilogue(Ctx& c, int k, int layer, int tile, c
       up[0][2 * i + 1] = u.y;
     }
   }
-  if (gq == 7 && c.warp < 7) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const float2 u = x2[(((c.warp + 1) * 2 + 1) * 4 + i) * 4 + t];
-      dn[1][2 * i] = u.x;
-      dn[1][2 * i + 1] = u.y;
-    }
-  }
   const int chunk_stride = g.rows_alloc * 8;           // halfs between k-chunks of an activation buffer
   float* const res0 = e.res + tile * (kTileM * kFeat);
   __half* const act0 = e.act + tile * (kTileOut * 8);
@@ -556,6 +558,21 @@ __device__ __forceinline__ int tc_epilogue(Ctx& c, int k, int layer, int tile, c
   int hit = 0;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
+    if (h == 1) {   // dn[1] of row m0 + 8 = 15 of the warp is D[m0 + 9][dx=+1]: row 0 of the next warp
+      if (c.warp == 3) {   // row 63 waits for warpgroup 1's row 64, i.e. for that warpgroup's MMAs of this tile
+        const long long ts = prof_now(c);
+        asm volatile("bar.sync %0, 64;" ::"n"(kBarSeamDn) : "memory");
+        if (c.lane == 0) prof_add(c, 23, prof_now(c) - ts);
+      }
+      if (gq == 7 && c.warp < 7) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float2 u = x2[(((c.warp + 1) * 2 + 1) * 4 + i) * 4 + t];
+          dn[1][2 * i] = u.x;
+          dn[1][2 * i + 1] = u.y;
+        }
+      }
+    }
     const int m = m0 + 8 * h;
     const int r = tile * kTileOut - 1 + m;             // FoV row of accumulator row m
     const unsigned f = flags >> (4 * h);
@@ -691,6 +708,25 @@ __device__ __forceinline__ void face_reduce(const Ctx& c, int k, int tb, int te,
   if (c.tid == 0) prof_add(c, 20, prof_now(c) - t0);
 }
 
+// The fp16 path's consumer warpgroups issue their tiles' MMAs in turn (each opens the other's turn as soon as its own
+// MMAs are issued): warpgroup 1's MMAs of a tile queue behind warpgroup 0's and run under warpgroup 0's epilogue of that
+// tile, and warpgroup 0's of the next tile under warpgroup 1's.  Warpgroup 0 issues tile i + 1 only after warpgroup 1
+// has issued tile i, so the skew between them stays below one tile: the neighbour exchange, double-buffered by tile
+// parity (epi_cnt), is enough.  Every warp still arrives once at `empty` after its own MMAs (8 arrivals), so the
+// producer's weight prefetch, implied by the kActStages-th `empty` wait of a layer, still follows every MMA of the
+// layer before.  publish_counts and face_reduce re-join the warpgroups once per chain and round; that only idles the
+// tensor cores for one tile.  Named barriers count arrivals, so a warpgroup must not arrive twice before the other has
+// synced: it arrives again only after its own next turn, which needs the other's arrival.  The turn of a
+// layers_pipelined call starts with warpgroup 1's arrival and ends with warpgroup 0 taking warpgroup 1's last one.
+__device__ __forceinline__ void order_wait(int wg) {   // until warpgroup `wg`'s turn
+  if (wg) asm volatile("bar.sync %0, 256;" ::"n"(kBarOrder0 + 1) : "memory");
+  else asm volatile("bar.sync %0, 256;" ::"n"(kBarOrder0) : "memory");
+}
+__device__ __forceinline__ void order_pass(int wg) {   // warpgroup `wg` hands the turn to the other one
+  if (wg) asm volatile("bar.arrive %0, 256;" ::"n"(kBarOrder0) : "memory");
+  else asm volatile("bar.arrive %0, 256;" ::"n"(kBarOrder0 + 1) : "memory");
+}
+
 // One round of the conv stacks of the chains in `mask`, as ONE warp-specialised pipeline over the work
 // items (layer, chain, tile) in that order:
 //   warp 8    TMA producer : waits for the chain's split-phase barrier (previous layer complete in every
@@ -786,7 +822,10 @@ __device__ __forceinline__ void layers_pipelined(Ctx& c, unsigned mask) {
       }
   } else {
     // ------------------------------------------------------------------ consumers (warps 0-7)
-    const uint32_t wg_rows = (uint32_t)((c.warp >> 2) * 64);   // this warpgroup's first accumulator row (16-byte units)
+    const int wg = c.warp >> 2;
+    const uint32_t wg_rows = (uint32_t)(wg * 64);   // this warpgroup's first accumulator row (16-byte units)
+    const bool wg_lead = (c.tid & 127) == 0;        // profiles its warpgroup
+    if (wg == 1) order_pass(1);   // warpgroup 0 goes first
     for (int layer = 0; layer < nconv; ++layer) {
       const int buf = layer & 1;
       long long t0 = prof_now(c);
@@ -806,25 +845,29 @@ __device__ __forceinline__ void layers_pipelined(Ctx& c, unsigned mask) {
           mbar_wait(c, &c.mb_full[s], (c.epi_cnt / kActStages) & 1u);
           if (c.tid == 0) prof_add(c, 1, prof_now(c) - t0);
           if (c.tid == 0) trace_ev(c, 2, c.epi_cnt);
-          t0 = prof_now(c);
           tc_prefetch_residual(c, e, layer, tile);   // lands in L1 while the MMAs run
           const uint32_t a_lo = (((sm90::smem_u32(act_smem + (size_t)s * stage_bytes) >> 4) & 0x3FFFu) + wg_rows) |
                                 ((uint32_t)(3 * seg_rows) << 16);
+          t0 = prof_now(c);
+          order_wait(wg);
+          if (wg_lead) prof_add(c, 24 + wg, prof_now(c) - t0);
+          t0 = prof_now(c);
           float d[kAccRegs];   // written by the tile's first MMA
           if (layer == 0) {
             tc_mma_issue<2>(d, a_lo, b_lo, seg_rows, g.xp, std::make_integer_sequence<int, 9>{});
           } else {
             tc_mma_issue<4>(d, a_lo, b_lo, seg_rows, g.xp, std::make_integer_sequence<int, 18>{});
           }
+          order_pass(wg);   // the other warpgroup's MMAs queue behind these
           const unsigned flags = tc_row_flags(c, tile);   // the load's latency runs under the MMAs
           sm90::wgmma_wait_all();
           __syncwarp();
           if (c.lane == 0) sm90::mbar_arrive(&c.mb_empty[s]);   // this warp's MMAs have read the stage
-          if (c.tid == 0) prof_add(c, 3, prof_now(c) - t0);
+          if (wg_lead) prof_add(c, wg ? 21 : 3, prof_now(c) - t0);
           if (c.tid == 0) trace_ev(c, 4, c.epi_cnt);
           t0 = prof_now(c);
           hit += tc_epilogue_any<false>(c, k, layer, tile, e, flags, d);
-          if (c.tid == 0) prof_add(c, 5, prof_now(c) - t0);
+          if (wg_lead) prof_add(c, wg ? 22 : 5, prof_now(c) - t0);
           if (c.tid == 0) trace_ev(c, 6, c.epi_cnt - 1u);
         }
         if (layer == nconv - 1) {
@@ -838,6 +881,7 @@ __device__ __forceinline__ void layers_pipelined(Ctx& c, unsigned mask) {
         }
       }
     }
+    if (wg == 0) order_wait(0);   // takes warpgroup 1's last arrival: none is left pending
   }
   // role-independent bookkeeping, identical in every thread (the weight-barrier parities, bits 0 / 1, are
   // tracked by the consumer warps alone: nobody else waits on those barriers)

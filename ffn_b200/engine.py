@@ -111,7 +111,8 @@ class Engine:
   PROFILE_SLOTS = ('barrier_wait', 'act_tma_wait', 'weight_wait', 'mma', 'unused4', 'epi_body',
                    'stage', 'paste', 'leader', 'steps', 'kernel', 'conv_layers', 'leader_policy', 'leader_pops',
                    'chain_barrier_wait', 'unused', 'leader_copy_in', 'leader_advance', 'leader_copy_out',
-                   'round_flag_wait', 'face_reduce') + ('unused',) * 11
+                   'round_flag_wait', 'face_reduce', 'mma_wg1', 'epi_body_wg1', 'seam_wait_warp3', 'order_wait_wg0',
+                   'order_wait_wg1') + ('unused',) * 6
 
   def enable_profiling(self, on: bool = True):
     _lib.check(self._lib.ffn_engine_profile(self._h, None, 1 if on else 0))
