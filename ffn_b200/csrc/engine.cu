@@ -49,16 +49,46 @@ int fail(const std::string& msg) {
                   std::to_string(__LINE__) + ")");                                             \
   } while (0)
 
-template <typename T>
-int dev_alloc(T** p, size_t n, bool zero = true) {
-  CUDA_OK(cudaMalloc(reinterpret_cast<void**>(p), std::max<size_t>(n, 1) * sizeof(T)));
-  if (zero) CUDA_OK(cudaMemset(*p, 0, std::max<size_t>(n, 1) * sizeof(T)));
-  return 0;
-}
+// The only owner of device memory: the temporaries of one call, or the buffers an engine or a canvas holds for its
+// lifetime.  It frees everything it allocated when it goes away, on every return path.  As a member of an engine or a
+// canvas it is destroyed after that object's destructor has made the object's device current.
+struct DevBufs {
+  std::vector<void*> p;
+  DevBufs() = default;
+  DevBufs(const DevBufs&) = delete;
+  DevBufs& operator=(const DevBufs&) = delete;
+  ~DevBufs() { for (void* q : p) cudaFree(q); }
+  // *out is set only when the allocation succeeds.
+  template <typename T>
+  int get(T** out, size_t count, bool zero = false) {
+    const size_t bytes = std::max<size_t>(count, 1) * sizeof(T);
+    void* q = nullptr;
+    CUDA_OK(cudaMalloc(&q, bytes));
+    p.push_back(q);
+    *out = static_cast<T*>(q);
+    if (zero) CUDA_OK(cudaMemset(q, 0, bytes));
+    return 0;
+  }
+  // Frees q (null: nothing) and sets it to null.
+  template <typename T>
+  void release(T*& q) {
+    p.erase(std::remove(p.begin(), p.end(), q), p.end());
+    cudaFree(q);
+    q = nullptr;
+  }
+};
 
 }  // namespace
 
 struct FfnEngine {
+  // Buffers: workspace, weights, tables, per-chain buffers and the predict staging.
+  DevBufs mem;
+  ~FfnEngine() {
+    cudaSetDevice(device);
+    cudaDeviceSynchronize();
+    if (ev0) cudaEventDestroy(ev0);
+    if (ev1) cudaEventDestroy(ev1);
+  }
   int device = 0;
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
@@ -83,7 +113,6 @@ struct FfnEngine {
   float* d_in_image = nullptr;
   float* d_out = nullptr;
   int predict_cap = 0;
-  std::vector<void*> owned;
   double last_kernel_seconds = 0.0;
   bool profiling = false;
   long long launches = 0;
@@ -95,12 +124,14 @@ struct FfnEngine {
 };
 
 struct FfnCanvas {
+  // Buffers: image, canvases, masks, event trace, object buffers and the snapshot array.
+  DevBufs mem;
+  ~FfnCanvas() { cudaSetDevice(eng->device); }
   FfnEngine* eng = nullptr;
   ffn::CanvasDev cv{};
   ffn::ObjDev ob[ffn::kMaxBufs]{};        // object buffers; [0] holds the canvas's own seed array
   int nbufs_alloc = 1;
   float* d_snap = nullptr;                // snapshot seed array (Sched::last_chain), allocated with the extra chains
-  std::vector<void*> pools;               // allocations behind object buffers 1.. and the snapshot array
   ffn::CanvasState* d_state = nullptr;    // [kMaxBufs]
   ffn::CanvasState h_state{};             // buffer 0
   ffn::Sched* d_sched = nullptr;
@@ -108,7 +139,7 @@ struct FfnCanvas {
   size_t q_cap = 0, traj_cap = 0;
   long long last_spec[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // last segment_all: early runs started / discarded / their steps / steps executed
   std::vector<int64_t> last_sched;        // last segment_all: ffn_canvas_sched_stats
-  void* d_image = nullptr;
+  uint8_t* d_image = nullptr;             // uint8 or float32 voxels (cv.image_is_u8)
   uint8_t* d_mask = nullptr;
   uint8_t* d_seed_mask = nullptr;
   float* d_pred = nullptr;
@@ -125,23 +156,6 @@ int set_device(const FfnEngine* e) {
   CUDA_OK(cudaSetDevice(e->device));
   return 0;
 }
-
-// Device allocations of one call, released on every return path.
-struct DevBufs {
-  std::vector<void*> p;
-  ~DevBufs() { for (void* q : p) cudaFree(q); }
-  template <typename T>
-  int get(T** out, size_t count, bool zero = false) {
-    if (dev_alloc(out, count, false)) return 1;
-    p.push_back(*out);
-    if (zero) CUDA_OK(cudaMemset(*out, 0, std::max<size_t>(count, 1) * sizeof(T)));
-    return 0;
-  }
-  void release(void* q) {
-    p.erase(std::remove(p.begin(), p.end(), q), p.end());
-    cudaFree(q);
-  }
-};
 
 // One temporary-storage buffer for all CUB calls of one entry point.  Each call is written once, as a callable
 // (void* temp, size_t& bytes) -> cudaError_t: alloc() queries every call's size (temp == nullptr) and allocates the
@@ -182,18 +196,6 @@ int use_device(int device, cudaDeviceProp* prop) {
                 "; this library only contains sm_90a code");
   CUDA_OK(cudaSetDevice(device));
   return 0;
-}
-
-void engine_free(FfnEngine* e) {
-  cudaSetDevice(e->device);
-  cudaDeviceSynchronize();
-  for (void* p : e->owned) cudaFree(p);
-  cudaFree(e->d_in_seed);
-  cudaFree(e->d_in_image);
-  cudaFree(e->d_out);
-  cudaEventDestroy(e->ev0);
-  cudaEventDestroy(e->ev1);
-  delete e;
 }
 
 Geom make_geom(const FfnModelDesc& m) {
@@ -295,23 +297,9 @@ int push_state(FfnCanvas* c) {
   return 0;
 }
 
-// Seed array, queue, done lattice and trajectory log of one object buffer (buffer 0's seed array is the canvas's own).
-int alloc_buf(FfnCanvas* c, int k) {
-  ObjDev& ch = c->ob[k];
-  if (k > 0) {
-    if (dev_alloc(&ch.seed, c->nvox, false)) return 1;
-    fill_f32_kernel<<<c->eng->sm_count * 8, 256, 0, cudaStreamPerThread>>>(ch.seed, c->nvox, NAN);
-    CUDA_OK(cudaGetLastError());
-  }
-  if (dev_alloc(&ch.lattice, c->lattice_cells)) return 1;
-  if (dev_alloc(&ch.q_score, c->q_cap, false)) return 1;
-  if (dev_alloc(&ch.q_pos, c->q_cap * 3, false)) return 1;
-  if (dev_alloc(&ch.traj, c->traj_cap * 3, false)) return 1;
-  return 0;
-}
-
 // Object buffers 1 .. n-1 and the snapshot array, on first use: ONE allocation for the seed arrays and one for the
-// small per-object arrays (two dozen separate cudaMalloc calls of 60 MB took 6 - 100 ms of a 2 s segment_all).
+// small per-object arrays, both owned by the canvas (two dozen separate cudaMalloc calls of 60 MB took 6 - 100 ms of a
+// 2 s segment_all).
 int ensure_bufs(FfnCanvas* c, int n) {
   const int first = c->nbufs_alloc;
   const bool need_snap = n > 1 && !c->d_snap;
@@ -325,14 +313,12 @@ int ensure_bufs(FfnCanvas* c, int n) {
   unsigned char *big = nullptr, *small = nullptr;
   const size_t big_total = seed_b * (size_t)(nnew + (need_snap ? 1 : 0));
   if (big_total) {
-    CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&big), big_total));
-    c->pools.push_back(big);
+    if (c->mem.get(&big, big_total)) return 1;
     fill_f32_kernel<<<c->eng->sm_count * 8, 256, 0, cudaStreamPerThread>>>(reinterpret_cast<float*>(big), big_total / sizeof(float), NAN);
     CUDA_OK(cudaGetLastError());
   }
   if (nnew) {
-    CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&small), small_b * (size_t)nnew));
-    c->pools.push_back(small);
+    if (c->mem.get(&small, small_b * (size_t)nnew)) return 1;
     CUDA_OK(cudaMemsetAsync(small, 0, small_b * (size_t)nnew, cudaStreamPerThread));
   }
   for (int i = 0; i < nnew; ++i) {
@@ -499,16 +485,13 @@ int ffn_engine_create(int device, const FfnModelDesc* model, const float* const*
   std::vector<__half> w16, w16x2;
   std::vector<float> w32;
   pack_weights(g, weights_dhwio, w16, w16x2, w32);
-  __half* d_w16 = nullptr;
-  __half* d_w16x2 = nullptr;
-  if (dev_alloc(&d_w16x2, w16x2.size())) return 1;
-  CUDA_OK(cudaMemcpy(d_w16x2, w16x2.data(), w16x2.size() * sizeof(__half), cudaMemcpyHostToDevice));
-  e->w.w16x2 = d_w16x2;
+  DevBufs& mem = e->mem;
+  __half *d_w16 = nullptr, *d_w16x2 = nullptr;
   float *d_w32 = nullptr, *d_bias = nullptr, *d_wlom = nullptr;
-  if (dev_alloc(&d_w16, w16.size())) return 1;
-  if (dev_alloc(&d_w32, w32.size())) return 1;
-  if (dev_alloc(&d_bias, (size_t)g.nconv * 32)) return 1;
-  if (dev_alloc(&d_wlom, 32)) return 1;
+  if (mem.get(&d_w16x2, w16x2.size(), true) || mem.get(&d_w16, w16.size(), true) || mem.get(&d_w32, w32.size(), true) ||
+      mem.get(&d_bias, (size_t)g.nconv * 32, true) || mem.get(&d_wlom, 32, true))
+    return 1;
+  CUDA_OK(cudaMemcpy(d_w16x2, w16x2.data(), w16x2.size() * sizeof(__half), cudaMemcpyHostToDevice));
   CUDA_OK(cudaMemcpy(d_w16, w16.data(), w16.size() * sizeof(__half), cudaMemcpyHostToDevice));
   CUDA_OK(cudaMemcpy(d_w32, w32.data(), w32.size() * sizeof(float), cudaMemcpyHostToDevice));
   std::vector<float> hb((size_t)g.nconv * 32);
@@ -516,35 +499,26 @@ int ffn_engine_create(int device, const FfnModelDesc* model, const float* const*
   CUDA_OK(cudaMemcpy(d_bias, hb.data(), hb.size() * sizeof(float), cudaMemcpyHostToDevice));
   CUDA_OK(cudaMemcpy(d_wlom, weights_dhwio[g.nconv], 32 * sizeof(float), cudaMemcpyHostToDevice));
   e->w.w16 = d_w16;
+  e->w.w16x2 = d_w16x2;
   e->w.w32 = d_w32;
   e->w.bias = d_bias;
   e->w.w_lom = d_wlom;
   e->w.b_lom = biases[g.nconv][0];
-  e->owned = {d_w16, d_w16x2, d_w32, d_bias, d_wlom};
 
   // workspace (all buffers zero-initialised: pad rows / guards must stay zero forever)
   Workspace& ws = e->ws;
   const size_t ra = (size_t)g.rows_alloc;
-  if (dev_alloc(&ws.act0_l, 2 * ra * 8)) return 1;
-  if (dev_alloc(&ws.act_l[0], 4 * ra * 8)) return 1;
-  if (dev_alloc(&ws.act_l[1], 4 * ra * 8)) return 1;
-  if (dev_alloc(&ws.act0_f, ra)) return 1;
-  if (dev_alloc(&ws.act_f[0], 8 * ra)) return 1;
-  if (dev_alloc(&ws.act_f[1], 8 * ra)) return 1;
-  if (dev_alloc(&ws.res, 8 * ra)) return 1;
-  if (dev_alloc(&ws.bar, 1)) return 1;
-  if (dev_alloc(&ws.abort_flag, 1)) return 1;
-  if (dev_alloc(&ws.prof, 2 * kProfSlots + kTraceEvents * kTraceTiles)) return 1;
-  for (void* p : std::vector<void*>{ws.act0_l, ws.act_l[0], ws.act_l[1], ws.act0_f, ws.act_f[0], ws.act_f[1], ws.res,
-                                    ws.bar, ws.abort_flag, ws.prof})
-    e->owned.push_back(p);
+  if (mem.get(&ws.act0_l, 2 * ra * 8, true) || mem.get(&ws.act_l[0], 4 * ra * 8, true) ||
+      mem.get(&ws.act_l[1], 4 * ra * 8, true) || mem.get(&ws.act0_f, ra, true) || mem.get(&ws.act_f[0], 8 * ra, true) ||
+      mem.get(&ws.act_f[1], 8 * ra, true) || mem.get(&ws.res, 8 * ra, true) || mem.get(&ws.bar, 1, true) ||
+      mem.get(&ws.abort_flag, 1, true) || mem.get(&ws.prof, 2 * kProfSlots + kTraceEvents * kTraceTiles, true))
+    return 1;
   {
     std::vector<uint8_t> flags((size_t)g.nt * 64);
     for (int t = 0; t < g.nt; ++t)
       for (int i = 0; i < 64; ++i) flags[(size_t)t * 64 + i] = row_flags_byte(g, t, i / 8, i % 8);
     uint8_t* d_flags = nullptr;
-    if (dev_alloc(&d_flags, flags.size())) return 1;
-    e->owned.push_back(d_flags);
+    if (mem.get(&d_flags, flags.size(), true)) return 1;
     CUDA_OK(cudaMemcpy(d_flags, flags.data(), flags.size(), cudaMemcpyHostToDevice));
     ws.row_flags = d_flags;
   }
@@ -554,10 +528,9 @@ int ffn_engine_create(int device, const FfnModelDesc* model, const float* const*
     build_face_table(g, tab, first);
     FaceEntry* d_tab = nullptr;
     int* d_first = nullptr;
-    if (dev_alloc(&d_tab, std::max<size_t>(tab.size(), 1))) return 1;
-    if (dev_alloc(&d_first, first.size())) return 1;
-    if (dev_alloc(&ws.face_best, (size_t)kMaxChains * kFaceSlots)) return 1;
-    for (void* p : std::vector<void*>{d_tab, d_first, ws.face_best}) e->owned.push_back(p);
+    if (mem.get(&d_tab, tab.size(), true) || mem.get(&d_first, first.size(), true) ||
+        mem.get(&ws.face_best, (size_t)kMaxChains * kFaceSlots, true))
+      return 1;
     CUDA_OK(cudaMemcpy(d_tab, tab.data(), tab.size() * sizeof(FaceEntry), cudaMemcpyHostToDevice));
     CUDA_OK(cudaMemcpy(d_first, first.data(), first.size() * sizeof(int), cudaMemcpyHostToDevice));
     ws.face_tab = d_tab;
@@ -565,18 +538,11 @@ int ffn_engine_create(int device, const FfnModelDesc* model, const float* const*
   }
   for (int k = 0; k < kMaxChains; ++k) {   // per-chain step workspace: fp16 operands, raw seed, logits, counters, barrier,
     ChainDev& cw = e->cws[k];              // fp32 residual stream
-    if (dev_alloc(&cw.act0_h, 2 * ra * 8)) return 1;
-    if (dev_alloc(&cw.act_h[0], 4 * ra * 8)) return 1;
-    if (dev_alloc(&cw.act_h[1], 4 * ra * 8)) return 1;
-    if (dev_alloc(&cw.seed_raw[0], (size_t)g.nt * kTileM)) return 1;
-    if (dev_alloc(&cw.seed_raw[1], (size_t)g.nt * kTileM)) return 1;
-    if (dev_alloc(&cw.logits, (size_t)g.nt * kTileM)) return 1;
-    if (dev_alloc(&cw.count, 4)) return 1;
-    if (dev_alloc(&cw.bar, 1)) return 1;
-    if (dev_alloc(&cw.res, (size_t)g.nt * kTileM * kFeat)) return 1;
-    for (void* p : std::vector<void*>{cw.act0_h, cw.act_h[0], cw.act_h[1], cw.seed_raw[0], cw.seed_raw[1], cw.logits,
-                                      cw.count, cw.bar, cw.res})
-      e->owned.push_back(p);
+    if (mem.get(&cw.act0_h, 2 * ra * 8, true) || mem.get(&cw.act_h[0], 4 * ra * 8, true) ||
+        mem.get(&cw.act_h[1], 4 * ra * 8, true) || mem.get(&cw.seed_raw[0], (size_t)g.nt * kTileM, true) ||
+        mem.get(&cw.seed_raw[1], (size_t)g.nt * kTileM, true) || mem.get(&cw.logits, (size_t)g.nt * kTileM, true) ||
+        mem.get(&cw.count, 4, true) || mem.get(&cw.bar, 1, true) || mem.get(&cw.res, (size_t)g.nt * kTileM * kFeat, true))
+      return 1;
   }
   // Tensor maps for the tile loads (driver entry point fetched at run time: no link-time dependency on libcuda).
   {
@@ -605,11 +571,9 @@ int ffn_engine_create(int device, const FfnModelDesc* model, const float* const*
     const char* env = std::getenv("FFN_B200_TMAP");
     e->use_tmap = (ok && env && std::atoi(env) != 0) ? 1 : 0;
   }
-  if (dev_alloc(&e->d_ctl, 1)) return 1;
-  if (dev_alloc(&e->d_round_flag, 1)) return 1;
-  if (dev_alloc(&e->d_dummy_state, kMaxBufs)) return 1;
-  if (dev_alloc(&e->d_dummy_sched, 1)) return 1;
-  for (void* p : std::vector<void*>{e->d_ctl, e->d_round_flag, e->d_dummy_state, e->d_dummy_sched}) e->owned.push_back(p);
+  if (mem.get(&e->d_ctl, 1, true) || mem.get(&e->d_round_flag, 1, true) || mem.get(&e->d_dummy_state, kMaxBufs, true) ||
+      mem.get(&e->d_dummy_sched, 1, true))
+    return 1;
   *out = e.release();
   return 0;
 }
@@ -620,7 +584,7 @@ void ffn_engine_destroy(FfnEngine* e) {
     e->closing = true;
     return;
   }
-  engine_free(e);
+  delete e;
 }
 
 int ffn_engine_set_grid(FfnEngine* e, int num_ctas) {
@@ -715,14 +679,12 @@ int ffn_predict(FfnEngine* e, const float* seed, const float* image, int batch, 
   if (!e || !seed || !image || !logits_out || batch < 1) return fail("bad argument");
   if (set_device(e)) return 1;
   const size_t n = (size_t)batch * e->g.V;
-  if (batch > e->predict_cap) {
-    cudaFree(e->d_in_seed);
-    cudaFree(e->d_in_image);
-    cudaFree(e->d_out);
-    e->d_in_seed = e->d_in_image = e->d_out = nullptr;
-    if (dev_alloc(&e->d_in_seed, n, false)) return 1;
-    if (dev_alloc(&e->d_in_image, n, false)) return 1;
-    if (dev_alloc(&e->d_out, n, false)) return 1;
+  if (batch > e->predict_cap) {   // no capacity until all three are reallocated: the next call retries a failed one
+    e->predict_cap = 0;
+    e->mem.release(e->d_in_seed);
+    e->mem.release(e->d_in_image);
+    e->mem.release(e->d_out);
+    if (e->mem.get(&e->d_in_seed, n) || e->mem.get(&e->d_in_image, n) || e->mem.get(&e->d_out, n)) return 1;
     e->predict_cap = batch;
   }
   CUDA_OK(cudaMemcpyAsync(e->d_in_seed, seed, n * sizeof(float), cudaMemcpyHostToDevice, cudaStreamPerThread));
@@ -769,14 +731,13 @@ int ffn_canvas_create(FfnEngine* e, const void* image, int image_dtype, const in
   cv.mean = image_mean;
   cv.stddev = image_stddev;
   const size_t ibytes = c->nvox * (cv.image_is_u8 ? 1 : 4);
-  CUDA_OK(cudaMalloc(&c->d_image, ibytes));
+  DevBufs& mem = c->mem;
+  if (mem.get(&c->d_image, ibytes)) return 1;
   CUDA_OK(cudaMemcpy(c->d_image, image, ibytes, cudaMemcpyHostToDevice));
   cv.image = c->d_image;
-  if (dev_alloc(&c->ob[0].seed, c->nvox, false)) return 1;
-  if (dev_alloc(&cv.seg, c->nvox)) return 1;
-  if (keep_probability_maps) {
-    if (dev_alloc(&cv.qprob, c->nvox)) return 1;
-  }
+  if (mem.get(&c->ob[0].seed, c->nvox) || mem.get(&cv.seg, c->nvox, true) ||
+      (keep_probability_maps && mem.get(&cv.qprob, c->nvox, true)))
+    return 1;
   fill_f32_kernel<<<e->sm_count * 8, 256, 0, cudaStreamPerThread>>>(c->ob[0].seed, c->nvox, NAN);
   CUDA_OK(cudaGetLastError());
   // movement policy storage
@@ -795,10 +756,11 @@ int ffn_canvas_create(FfnEngine* e, const void* image, int image_dtype, const in
   c->traj_cap = std::min<size_t>(qcells + 16, (size_t)1 << 28);   // one FoV step per lattice cell at most
   cv.q_cap = (int)c->q_cap;
   cv.traj_cap = (int)c->traj_cap;
-  if (alloc_buf(c.get(), 0)) return 1;
-  if (dev_alloc(&c->d_state, kMaxBufs)) return 1;
-  if (dev_alloc(&c->d_sched, 1)) return 1;
-  if (dev_alloc(&c->d_pred, (size_t)g.V, false)) return 1;
+  ObjDev& ob0 = c->ob[0];   // buffer 0's movement queue, done lattice and trajectory log
+  if (mem.get(&ob0.lattice, c->lattice_cells, true) || mem.get(&ob0.q_score, c->q_cap) || mem.get(&ob0.q_pos, c->q_cap * 3) ||
+      mem.get(&ob0.traj, c->traj_cap * 3) || mem.get(&c->d_state, kMaxBufs, true) || mem.get(&c->d_sched, 1, true) ||
+      mem.get(&c->d_pred, (size_t)g.V))
+    return 1;
   std::memset(&c->h_state, 0, sizeof(CanvasState));
   std::memset(&c->h_sched, 0, sizeof(Sched));
   c->h_sched.owner = -1;
@@ -820,24 +782,8 @@ int ffn_canvas_create(FfnEngine* e, const void* image, int image_dtype, const in
 void ffn_canvas_destroy(FfnCanvas* c) {
   if (!c) return;
   FfnEngine* e = c->eng;
-  cudaSetDevice(e->device);
-  cudaFree(c->d_image);
-  cudaFree(c->ob[0].seed);      // buffer 0 is allocated with the canvas; the others and the snapshot array live in pools
-  cudaFree(c->ob[0].lattice);
-  cudaFree(c->ob[0].q_score);
-  cudaFree(c->ob[0].q_pos);
-  cudaFree(c->ob[0].traj);
-  for (void* q : c->pools) cudaFree(q);
-  cudaFree(c->cv.seg);
-  cudaFree(c->cv.qprob);
-  cudaFree(c->cv.trace);
-  cudaFree(c->d_state);
-  cudaFree(c->d_sched);
-  cudaFree(c->d_pred);
-  cudaFree(c->d_mask);
-  cudaFree(c->d_seed_mask);
   delete c;
-  if (--e->live_canvases == 0 && e->closing) engine_free(e);
+  if (--e->live_canvases == 0 && e->closing) delete e;
 }
 
 int ffn_canvas_set_mask(FfnCanvas* c, int which, const uint8_t* mask) {
@@ -846,10 +792,9 @@ int ffn_canvas_set_mask(FfnCanvas* c, int which, const uint8_t* mask) {
   uint8_t** slot = which == FFN_MASK_MOVEMENT ? &c->d_mask : which == FFN_MASK_SEED ? &c->d_seed_mask : nullptr;
   if (!slot) return fail("unknown mask id");
   if (!mask) {
-    cudaFree(*slot);
-    *slot = nullptr;
+    c->mem.release(*slot);
   } else {
-    if (!*slot) CUDA_OK(cudaMalloc(reinterpret_cast<void**>(slot), c->nvox));
+    if (!*slot && c->mem.get(slot, c->nvox)) return 1;
     CUDA_OK(cudaMemcpy(*slot, mask, c->nvox, cudaMemcpyHostToDevice));
   }
   c->cv.mask = c->d_mask;
@@ -1299,11 +1244,10 @@ int ffn_canvas_trace(FfnCanvas* c, int64_t capacity, int32_t* events_out, int64_
     if (n > 0) CUDA_OK(cudaMemcpy(events_out, c->cv.trace, (size_t)n * 4 * sizeof(int), cudaMemcpyDeviceToHost));
     return 0;
   }
-  cudaFree(c->cv.trace);
-  c->cv.trace = nullptr;
+  c->mem.release(c->cv.trace);
   c->cv.trace_cap = 0;
   if (capacity > 0) {
-    if (dev_alloc(&c->cv.trace, (size_t)capacity * 4)) return 1;
+    if (c->mem.get(&c->cv.trace, (size_t)capacity * 4, true)) return 1;
     c->cv.trace_cap = (int)capacity;
   }
   c->h_state.n_trace = 0;
@@ -2337,10 +2281,62 @@ int ffn_clean_up(int device, const FfnCleanUpDesc* desc, uint64_t* labels, uint6
   return 0;
 }
 
+// D = A * B^T through selftest::wgmma_kat_kernel on small-integer operands, exact in fp32: out[0..2] are the worst
+// errors with A shifted by 0, 3 and 35 rows (0 expected), out[3] the one with LBO and SBO swapped (large expected), and
+// the other slots -1.
 int ffn_selftest_wgmma(int device, double* out, int n_out) {
   if (!out || n_out < 8) return fail("need >= 8 output slots");
-  std::string err;
-  if (ffn::selftest::run(device, out, n_out, &err)) return fail(err);
+  cudaDeviceProp prop{};
+  if (use_device(device, &prop)) return 1;
+  for (int i = 0; i < n_out; ++i) out[i] = -1.0;
+  const int K = 64, kch = K / 8, rows_total = 256;   // A window has room for shifts up to 127 rows
+  std::vector<float> a((size_t)rows_total * K), b((size_t)96 * K);
+  unsigned s = 12345u;
+  auto rnd = [&]() {
+    s = s * 1664525u + 1013904223u;
+    return (float)((int)((s >> 20) & 15) - 8) * 0.125f;
+  };
+  for (auto& v : a) v = rnd();
+  for (auto& v : b) v = rnd();
+  std::vector<__half> ah((size_t)kch * rows_total * 8), bh((size_t)kch * 96 * 8);
+  for (int r = 0; r < rows_total; ++r)
+    for (int k = 0; k < K; ++k) ah[((size_t)(k / 8) * rows_total + r) * 8 + k % 8] = __float2half_rn(a[(size_t)r * K + k]);
+  for (int n = 0; n < 96; ++n)
+    for (int k = 0; k < K; ++k)
+      bh[(((size_t)(k / 8)) * 12 + n / 8) * 64 + (n % 8) * 8 + k % 8] = __float2half_rn(b[(size_t)n * K + k]);
+  DevBufs bufs;
+  __half *d_a = nullptr, *d_b = nullptr;
+  float* d_d = nullptr;
+  if (bufs.get(&d_a, ah.size()) || bufs.get(&d_b, bh.size()) || bufs.get(&d_d, 128 * 96)) return 1;
+  CUDA_OK(cudaMemcpy(d_a, ah.data(), ah.size() * 2, cudaMemcpyHostToDevice));
+  CUDA_OK(cudaMemcpy(d_b, bh.data(), bh.size() * 2, cudaMemcpyHostToDevice));
+  // the swapped-descriptor case strides 8-row groups by a_lbo / b_lbo and reaches ~58 KB past the operand base:
+  // allocate that much so the wrong answer is a wrong number, not an out-of-range shared-memory read
+  const int smem = 64 * 1024;
+  CUDA_OK(cudaFuncSetAttribute(selftest::wgmma_kat_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  const uint32_t a_lbo = rows_total * 16, a_sbo = 128, b_lbo = 12 * 128, b_sbo = 128;
+  struct Case { int shift; bool swapped; };
+  const Case cases[4] = {{0, false}, {3, false}, {35, false}, {0, true}};
+  for (int ci = 0; ci < 4; ++ci) {
+    const Case& c = cases[ci];
+    CUDA_OK(cudaMemset(d_d, 0xff, 128 * 96 * 4));
+    selftest::wgmma_kat_kernel<<<1, 256, smem>>>(d_a, rows_total, d_b, kch, c.shift, c.swapped ? a_sbo : a_lbo,
+                                                 c.swapped ? a_lbo : a_sbo, c.swapped ? b_sbo : b_lbo,
+                                                 c.swapped ? b_lbo : b_sbo, d_d);
+    CUDA_OK(cudaGetLastError());
+    CUDA_OK(cudaDeviceSynchronize());
+    std::vector<float> d(128 * 96);
+    CUDA_OK(cudaMemcpy(d.data(), d_d, d.size() * 4, cudaMemcpyDeviceToHost));
+    double worst = 0;
+    for (int r = 0; r < 128; ++r)
+      for (int n = 0; n < 96; ++n) {
+        double ref = 0;
+        for (int k = 0; k < K; ++k) ref += (double)a[(size_t)(r + c.shift) * K + k] * (double)b[(size_t)n * K + k];
+        const double e = std::fabs(ref - (double)d[(size_t)r * 96 + n]);
+        if (!(e <= worst)) worst = std::isnan(e) ? 1e30 : e;
+      }
+    out[ci] = worst;
+  }
   return 0;
 }
 

@@ -446,7 +446,7 @@ int ffn_clean_up(int device, const FfnCleanUpDesc* desc, uint64_t* labels, uint6
                  int64_t* counts, int64_t cap, int64_t* n_ids);
 
 /* Known-answer test of the wgmma descriptors (worst absolute error of each case in out[]; see
- * ffn_b200/csrc/selftest.cuh).  Used by tests, not by the product path. */
+ * ffn_selftest_wgmma in ffn_b200/csrc/engine.cu).  Used by tests, not by the product path. */
 int ffn_selftest_wgmma(int device, double* out, int n_out);
 
 #ifdef __cplusplus
