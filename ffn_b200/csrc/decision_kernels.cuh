@@ -14,6 +14,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../../include/ffn_b200.h"
+
 namespace ffn {
 namespace dpk {
 

@@ -1,5 +1,5 @@
-// engine.cu — host side of libffn_b200.so: device context, weight packing, canvases, launches,
-// and the extern "C" entry points declared in include/ffn_b200.h.
+// engine.cu — host side of the flood engine: device context, weight packing, canvases, launches, their extern "C"
+// entry points declared in include/ffn_b200.h, and the library's last error (fail, ffn_last_error).
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
@@ -10,79 +10,79 @@
 #include <vector>
 
 #include "device_types.cuh"
-// the persistent kernel, twice: the product build and one with device cycle counters
-#define FFN_KNS plain
-#define FFN_PROFILE 0
-#include "flood_kernel.cuh"
-#undef FFN_KNS
-#undef FFN_PROFILE
-#define FFN_KNS profiled
-#define FFN_PROFILE 1
-#include "flood_kernel.cuh"
-#undef FFN_KNS
-#undef FFN_PROFILE
+#include "host.cuh"
 #include "seed_kernels.cuh"
-#include "decision_kernels.cuh"
-#include "reseg_kernels.cuh"
-#include "consensus_kernels.cuh"
-#include "partition_kernels.cuh"
-#include "coordinate_kernels.cuh"
-#include "cc_kernels.cuh"
-#include "selftest.cuh"
 
-#include <cub/cub.cuh>
+namespace ffn {
+
+// Adds `offset` to every label > 0 (multi-GPU merge, SURVEY.md 8e). HBM-bound, grid-stride.
+__global__ void relabel_offset_kernel(int* seg, size_t n, int offset) {
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const int v = seg[i];
+    if (v > 0) seg[i] = v + offset;
+  }
+}
+
+// u8 -> normalised float32 (runner.py:383-385), for ffn_canvas_read(FFN_ARRAY_IMAGE).
+__global__ void normalize_u8_kernel(const uint8_t* src, float* dst, size_t n, float mean, float stddev) {
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
+    dst[i] = __fdiv_rn(__fsub_rn((float)src[i], mean), stddev);
+}
+
+__global__ void fill_f32_kernel(float* dst, size_t n, float v) {
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) dst[i] = v;
+}
+
+// NaN-fill of a box (lo, size) of a float canvas: Canvas.init_seed's clear restricted to the touched box.
+__global__ void fill_box_f32_kernel(float* dst, int sy, int sx, int lz, int ly, int lx, int nz, int ny, int nx, float v) {
+  const size_t n = (size_t)nz * ny * nx;
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const int x = (int)(i % nx), y = (int)((i / nx) % ny), z = (int)(i / ((size_t)nx * ny));
+    dst[((size_t)(lz + z) * sy + (ly + y)) * sx + (lx + x)] = v;
+  }
+}
+
+// dst box <- src box (same canvas geometry): moves the last object's seed values into the canvas's own array.
+__global__ void copy_box_f32_kernel(float* dst, const float* src, int sy, int sx, int lz, int ly, int lx, int nz, int ny,
+                                    int nx) {
+  const size_t n = (size_t)nz * ny * nx;
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const int x = (int)(i % nx), y = (int)((i / nx) % ny), z = (int)(i / ((size_t)nx * ny));
+    const size_t a = ((size_t)(lz + z) * sy + (ly + y)) * sx + (lx + x);
+    dst[a] = src[a];
+  }
+}
+
+// The persistent kernel, one translation unit per build: flood_plain.cu (the product kernel) and flood_profiled.cu
+// (with device cycle counters).  `split` selects the split-fp16 instance over the fp16 / fp32 one.
+namespace plain {
+const void* flood_kernel(bool split);
+}
+namespace profiled {
+const void* flood_kernel(bool split);
+}
+
+}  // namespace ffn
 
 namespace {
 
 thread_local std::string g_error;
 
-int fail(const std::string& msg) {
+}  // namespace
+
+int ffn::fail(const std::string& msg) {
   g_error = msg;
   return 1;
 }
 
-#define CUDA_OK(expr)                                                                          \
-  do {                                                                                         \
-    cudaError_t e__ = (expr);                                                                  \
-    if (e__ != cudaSuccess)                                                                    \
-      return fail(std::string(#expr) + ": " + cudaGetErrorString(e__) + " (" + __FILE__ + ":" + \
-                  std::to_string(__LINE__) + ")");                                             \
-  } while (0)
-
-// The only owner of device memory: the temporaries of one call, or the buffers an engine or a canvas holds for its
-// lifetime.  It frees everything it allocated when it goes away, on every return path.  As a member of an engine or a
-// canvas it is destroyed after that object's destructor has made the object's device current.
-struct DevBufs {
-  std::vector<void*> p;
-  DevBufs() = default;
-  DevBufs(const DevBufs&) = delete;
-  DevBufs& operator=(const DevBufs&) = delete;
-  ~DevBufs() { for (void* q : p) cudaFree(q); }
-  // *out is set only when the allocation succeeds.
-  template <typename T>
-  int get(T** out, size_t count, bool zero = false) {
-    const size_t bytes = std::max<size_t>(count, 1) * sizeof(T);
-    void* q = nullptr;
-    CUDA_OK(cudaMalloc(&q, bytes));
-    p.push_back(q);
-    *out = static_cast<T*>(q);
-    if (zero) CUDA_OK(cudaMemset(q, 0, bytes));
-    return 0;
-  }
-  // Frees q (null: nothing) and sets it to null.
-  template <typename T>
-  void release(T*& q) {
-    p.erase(std::remove(p.begin(), p.end(), q), p.end());
-    cudaFree(q);
-    q = nullptr;
-  }
-};
-
-}  // namespace
-
 struct FfnEngine {
   // Buffers: workspace, weights, tables, per-chain buffers and the predict staging.
-  DevBufs mem;
+  ffn::DevBufs mem;
   ~FfnEngine() {
     cudaSetDevice(device);
     cudaDeviceSynchronize();
@@ -125,7 +125,7 @@ struct FfnEngine {
 
 struct FfnCanvas {
   // Buffers: image, canvases, masks, event trace, object buffers and the snapshot array.
-  DevBufs mem;
+  ffn::DevBufs mem;
   ~FfnCanvas() { cudaSetDevice(eng->device); }
   FfnEngine* eng = nullptr;
   ffn::CanvasDev cv{};
@@ -154,47 +154,6 @@ using namespace ffn;
 
 int set_device(const FfnEngine* e) {
   CUDA_OK(cudaSetDevice(e->device));
-  return 0;
-}
-
-// One temporary-storage buffer for all CUB calls of one entry point.  Each call is written once, as a callable
-// (void* temp, size_t& bytes) -> cudaError_t: alloc() queries every call's size (temp == nullptr) and allocates the
-// largest, and run() runs one call against that buffer.  The sizes are queried at the calls' upper bounds on the item
-// count; CUB refuses a run that needs more than it is given.
-struct CubTemp {
-  char* p = nullptr;
-  size_t bytes = 0;
-  template <typename... F>
-  int alloc(DevBufs& bufs, const F&... calls) {
-    if ((size_for(calls) || ...)) return 1;
-    return bufs.get(&p, bytes);
-  }
-  template <typename F>
-  int size_for(const F& call) {
-    size_t b = 0;
-    CUDA_OK(call(nullptr, b));
-    bytes = std::max(bytes, b);
-    return 0;
-  }
-  template <typename F>
-  cudaError_t run(const F& call) const {
-    size_t b = bytes;
-    return call(p, b);
-  }
-};
-
-// The library only contains sm_90a code: every entry point that takes a device index accepts an sm_90 device only.
-// On success the device is the calling thread's current device and *prop holds its properties.
-int use_device(int device, cudaDeviceProp* prop) {
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
-    return fail("no CUDA device: libffn_b200 has no CPU fallback");
-  if (device < 0 || device >= ndev) return fail("bad device index");
-  CUDA_OK(cudaGetDeviceProperties(prop, device));
-  if (prop->major != 9 || prop->minor != 0)
-    return fail(std::string("device is sm_") + std::to_string(prop->major) + std::to_string(prop->minor) +
-                "; this library only contains sm_90a code");
-  CUDA_OK(cudaSetDevice(device));
   return 0;
 }
 
@@ -228,13 +187,12 @@ Geom make_geom(const FfnModelDesc& m) {
 int chain_limit(const FfnEngine* e) { return std::max(1, std::min(e->max_chains, (int)kMaxChains)); }
 
 // The flood kernel instances: {plain, profiled} x {fp16 / fp32, split fp16}.
-const void* const kFloodKernels[2][2] = {
-    {reinterpret_cast<const void*>(plain::ffn_flood_kernel<false>), reinterpret_cast<const void*>(plain::ffn_flood_kernel<true>)},
-    {reinterpret_cast<const void*>(profiled::ffn_flood_kernel<false>),
-     reinterpret_cast<const void*>(profiled::ffn_flood_kernel<true>)}};
+const void* flood_kernel(bool profiling, bool split) {
+  return profiling ? profiled::flood_kernel(split) : plain::flood_kernel(split);
+}
 
 const void* flood_kernel(const FfnEngine* e) {
-  return kFloodKernels[e->profiling ? 1 : 0][e->compute_mode == FFN_COMPUTE_FP16X2_TC ? 1 : 0];
+  return flood_kernel(e->profiling, e->compute_mode == FFN_COMPUTE_FP16X2_TC);
 }
 
 // Launches the persistent kernel once and waits for it.  `c` may be null (predict).
@@ -470,8 +428,9 @@ int ffn_engine_create(int device, const FfnModelDesc* model, const float* const*
   e->smem_bytes = L.total;
   if ((size_t)L.total > prop.sharedMemPerBlockOptin)
     return fail("field of view too large for the shared-memory operand staging");
-  for (const auto& by_mode : kFloodKernels)
-    for (const void* k : by_mode) {
+  for (const bool profiling : {false, true})
+    for (const bool split : {false, true}) {
+      const void* k = flood_kernel(profiling, split);
       CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total));
       int per_sm = 0;
       CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, kThreads, L.total));
@@ -1422,921 +1381,6 @@ int ffn_canvas_add_id_offset(FfnCanvas* c, int32_t offset) {
   relabel_offset_kernel<<<c->eng->sm_count * 8, 256, 0, cudaStreamPerThread>>>(c->cv.seg, c->nvox, offset);
   CUDA_OK(cudaGetLastError());
   CUDA_OK(cudaStreamSynchronize(cudaStreamPerThread));
-  return 0;
-}
-
-int ffn_decision_points(int device, const FfnDecisionPointDesc* desc, uint64_t* labels, FfnDecisionPoint* out,
-                        int64_t cap, int64_t* n_out) {
-  using dpk::u64;
-  if (!desc || !labels || !n_out || cap < 0 || (cap > 0 && !out)) return fail("bad argument");
-  const int sz = desc->shape_zyx[0], sy = desc->shape_zyx[1], sx = desc->shape_zyx[2];
-  if (sz < 1 || sy < 1 || sx < 1) return fail("shape must be positive");
-  const size_t n = (size_t)sz * sy * sx;
-  if (n >= (1ull << 31)) return fail("decision points support volumes of fewer than 2^31 voxels");
-  const int w[3] = {desc->voxel_size_xyz[2], desc->voxel_size_xyz[1], desc->voxel_size_xyz[0]};   // z, y, x
-  for (int a = 0; a < 3; ++a) {
-    if (w[a] < 1) return fail("voxel sizes must be positive integers");
-    if (desc->box_start_zyx[a] < 0 || desc->box_size_zyx[a] < 0 ||
-        (int64_t)desc->box_start_zyx[a] + desc->box_size_zyx[a] > desc->shape_zyx[a])
-      return fail("subvolume box lies outside the volume");
-  }
-  cudaDeviceProp prop{};
-  if (use_device(device, &prop)) return 1;
-  cudaStream_t st = cudaStreamPerThread;
-  const int blocks = prop.multiProcessorCount * 16;
-  DevBufs bufs;
-
-  // Compaction: sorted unique ids and their counts; the kept ids (non-zero, not dust) in uint64 order.
-  u64 *d_lab = nullptr, *d_sorted = nullptr, *d_unique = nullptr;
-  unsigned* d_counts = nullptr;
-  unsigned char* d_flags = nullptr;
-  int* d_num = nullptr;   // [0] runs, [1] kept ids
-  int nruns = (int)n;     // an upper bound until the run-length encoding has counted them
-  if (bufs.get(&d_lab, n) || bufs.get(&d_sorted, n) || bufs.get(&d_unique, n) || bufs.get(&d_counts, n) ||
-      bufs.get(&d_num, 2))
-    return 1;
-  u64* const d_kept = d_sorted;   // the sorted copy is no longer needed once the runs are encoded
-  auto sort = [&](void* t, size_t& b) {
-    return cub::DeviceRadixSort::SortKeys(t, b, d_lab, d_sorted, (int)n, 0, 64, st);
-  };
-  auto rle = [&](void* t, size_t& b) {
-    return cub::DeviceRunLengthEncode::Encode(t, b, d_sorted, d_unique, d_counts, d_num, (int)n, st);
-  };
-  auto select = [&](void* t, size_t& b) {
-    return cub::DeviceSelect::Flagged(t, b, d_unique, d_flags, d_kept, d_num + 1, nruns, st);
-  };
-  CubTemp temp;
-  if (temp.alloc(bufs, sort, rle, select)) return 1;
-  CUDA_OK(cudaMemcpyAsync(d_lab, labels, n * sizeof(u64), cudaMemcpyHostToDevice, st));
-  CUDA_OK(temp.run(sort));
-  CUDA_OK(temp.run(rle));
-  u64 first_id = 0;
-  CUDA_OK(cudaMemcpyAsync(&nruns, d_num, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaMemcpyAsync(&first_id, d_unique, sizeof(u64), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  if (bufs.get(&d_flags, nruns)) return 1;
-  dpk::flag_kept<<<blocks, 256, 0, st>>>(d_unique, d_counts, nruns, desc->dust_threshold, d_flags);
-  CUDA_OK(temp.run(select));
-  int nkept = 0;
-  CUDA_OK(cudaMemcpyAsync(&nkept, d_num + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  bufs.release(d_unique);
-  bufs.release(d_counts);
-  bufs.release(temp.p);
-  bufs.release(d_flags);
-  const bool dust_cleared = nkept < nruns - (first_id == 0 ? 1 : 0);
-
-  // Key range: every finite key (D + 1) * M - 1 must stay below kInf.
-  int log_m = 0;
-  while ((1ull << log_m) <= (u64)nkept) ++log_m;
-  const u64 m = 1ull << log_m;
-  unsigned __int128 dmax = 0;
-  for (int a = 0; a < 3; ++a) {
-    const unsigned __int128 e = (unsigned __int128)w[a] * (unsigned __int128)(desc->shape_zyx[a] - 1);
-    dmax += e * e;
-  }
-  if (dmax >= ((unsigned __int128)1 << 64) || ((dmax + 1) << log_m) >= ((unsigned __int128)1 << 64))
-    return fail("voxel size and extent too large for exact 64-bit distance keys: (D_max + 1) * M = (" +
-                std::to_string((double)dmax) + " + 1) * " + std::to_string(m) + " does not fit in 64 bits");
-
-  u64 *keys = nullptr, *keys2 = nullptr;
-  if (bufs.get(&keys, n)) return 1;
-  dpk::init_keys<<<blocks, 256, 0, st>>>(d_lab, d_kept, nkept, keys, n);
-  CUDA_OK(cudaGetLastError());
-  if (dust_cleared) CUDA_OK(cudaMemcpyAsync(labels, d_lab, n * sizeof(u64), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  bufs.release(d_lab);
-  *n_out = 0;
-  dpk::PairGeom g{};
-  for (int a = 0; a < 3; ++a) {
-    g.lo[a] = desc->box_start_zyx[a];
-    g.size[a] = desc->box_size_zyx[a];
-  }
-  if (nkept == 0 || (size_t)g.size[0] * g.size[1] * g.size[2] == 0) return 0;
-
-  // Exact nearest-id transform: x sweeps in place, then y (keys -> keys2) and z (keys2 -> keys).
-  int *sbuf = nullptr, *tbuf = nullptr;
-  if (bufs.get(&keys2, n) || bufs.get(&sbuf, n) || bufs.get(&tbuf, n)) return 1;
-  dpk::nid_x<<<blocks, 128, 0, st>>>(keys, sz, sy, sx, m * (u64)w[2] * (u64)w[2], m);
-  dpk::nid_line<<<blocks, 128, 0, st>>>(keys, keys2, 1, sz, sy, sx, m * (u64)w[1] * (u64)w[1], sbuf, tbuf);
-  dpk::nid_line<<<blocks, 128, 0, st>>>(keys2, keys, 0, sz, sy, sx, m * (u64)w[0] * (u64)w[0], sbuf, tbuf);
-  CUDA_OK(cudaGetLastError());
-  CUDA_OK(cudaStreamSynchronize(st));
-  bufs.release(keys2);
-  bufs.release(sbuf);
-  bufs.release(tbuf);
-
-  // Pair search; a table that fills up is discarded and rebuilt four times larger.
-  g.sy = sy;
-  g.sx = sx;
-  g.m = m;
-  g.log_m = log_m;
-  g.use_max_distance = desc->use_max_distance;
-  g.max_distance = desc->max_distance;
-  dpk::PairTable t{};
-  u64* tmem = nullptr;
-  u64* d_misc = nullptr;   // [0] reserved slots, [1] overflow flag, [2] emitted pairs
-  if (bufs.get(&d_misc, 3)) return 1;
-  for (u64 tcap = 4096;; tcap *= 4) {
-    if (bufs.get(&tmem, 8 * tcap)) return 1;
-    t.key = tmem;
-    t.dist = tmem + tcap;
-    t.cnt = tmem + 2 * tcap;
-    t.sum = tmem + 3 * tcap;
-    t.c2 = tmem + 6 * tcap;
-    t.ord = tmem + 7 * tcap;
-    t.cap = tcap;
-    t.limit = tcap / 2;
-    t.used = d_misc;
-    t.overflow = (int*)(d_misc + 1);
-    CUDA_OK(cudaMemsetAsync(d_misc, 0, 3 * sizeof(u64), st));
-    dpk::table_init<<<blocks, 256, 0, st>>>(t);
-    dpk::pair_pass<1><<<blocks, 256, 0, st>>>(keys, g, t);
-    CUDA_OK(cudaGetLastError());
-    u64 misc[2] = {0, 0};
-    CUDA_OK(cudaMemcpyAsync(misc, d_misc, sizeof(misc), cudaMemcpyDeviceToHost, st));
-    CUDA_OK(cudaStreamSynchronize(st));
-    if (misc[1] == 0) break;
-    bufs.release(tmem);
-  }
-  dpk::pair_pass<2><<<blocks, 256, 0, st>>>(keys, g, t);
-  dpk::pair_pass<3><<<blocks, 256, 0, st>>>(keys, g, t);
-  dpk::pair_pass<4><<<blocks, 256, 0, st>>>(keys, g, t);
-  FfnDecisionPoint* d_out = nullptr;
-  if (bufs.get(&d_out, t.limit)) return 1;
-  dpk::emit_pairs<<<blocks, 256, 0, st>>>(t, d_kept, g.size[1], g.size[2], d_out, d_misc + 2);
-  CUDA_OK(cudaGetLastError());
-  u64 npairs = 0;
-  CUDA_OK(cudaMemcpyAsync(&npairs, d_misc + 2, sizeof(u64), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  std::vector<FfnDecisionPoint> host(npairs);
-  CUDA_OK(cudaMemcpyAsync(host.data(), d_out, npairs * sizeof(FfnDecisionPoint), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  std::sort(host.begin(), host.end(), [](const FfnDecisionPoint& p, const FfnDecisionPoint& q) {
-    return p.id_a < q.id_a || (p.id_a == q.id_a && p.id_b < q.id_b);
-  });
-  *n_out = (int64_t)npairs;
-  std::copy(host.begin(), host.begin() + std::min<int64_t>(cap, (int64_t)npairs), out);
-  return 0;
-}
-
-int ffn_reseg_eval(int device, const FfnResegEvalDesc* desc, const uint64_t* labels, const uint8_t* probs,
-                   const uint64_t* ids, const uint8_t mask_table[256], FfnResegStats* stats_out,
-                   FfnResegOverlap* overlaps_out, int64_t cap, int64_t* n_overlaps) {
-  using rsk::u64;
-  if (!desc || !n_overlaps || !stats_out || cap < 0 || (cap > 0 && !overlaps_out) || desc->num_items < 0 ||
-      (desc->num_items > 0 && (!labels || !probs || !ids || !mask_table)))
-    return fail("bad argument");
-  const int bz = desc->box_zyx[0], by = desc->box_zyx[1], bx = desc->box_zyx[2];
-  if (bz < 1 || by < 1 || bx < 1) return fail("box extent must be positive");
-  const long long nitems = desc->num_items, nbox = (long long)bz * by * bx;
-  const bool pair = desc->pair != 0;
-  if (nitems > 0 && nbox > ((1ll << 31) - 1) / (nitems * (pair ? 4 : 1)))
-    return fail("resegmentation analysis supports batches of fewer than 2^31 mask voxels (four masks per pair item)");
-  const int w[3] = {desc->voxel_size_zyx[0], desc->voxel_size_zyx[1], desc->voxel_size_zyx[2]};
-  unsigned __int128 dmax = 0;   // covers the no-background value, which uses the full z extent
-  for (int a = 0; a < 3; ++a) {
-    if (pair && w[a] < 1) return fail("voxel sizes must be positive integers");
-    const unsigned __int128 e = (unsigned __int128)(pair ? w[a] : 0) * (unsigned __int128)desc->box_zyx[a];
-    dmax += e * e;
-  }
-  if (dmax >= ((unsigned __int128)1 << 63)) return fail("voxel size and box too large for exact 64-bit squared distances");
-  *n_overlaps = 0;
-  if (nitems == 0) return 0;
-  cudaDeviceProp prop{};
-  if (use_device(device, &prop)) return 1;
-  cudaStream_t st = cudaStreamPerThread;
-  const int blocks = prop.multiProcessorCount * 16;
-  // Items (grid y) x blocks per box (grid x): about 16 resident blocks per SM over the whole batch.
-  const dim3 item_grid((unsigned)std::max<long long>(1, std::min<long long>((nbox + 1023) / 1024,
-                                                                              std::max<long long>(1, blocks / nitems))),
-                       (unsigned)std::min<long long>(nitems, 65535));
-  const size_t n = (size_t)(nitems * nbox);
-  const int nprob = pair ? 2 : 1;
-  DevBufs bufs;
-  u64 *d_lab = nullptr, *d_ids = nullptr, *d_counts = nullptr;
-  unsigned char *d_probs = nullptr, *d_table = nullptr;
-  const int ncounts = pair ? rsk::kPairCounts : 2;
-  if (bufs.get(&d_lab, n) || bufs.get(&d_probs, n * nprob) || bufs.get(&d_table, 256) ||
-      bufs.get(&d_counts, (size_t)nitems * ncounts) || bufs.get(&d_ids, 2 * nitems))
-    return 1;
-  CUDA_OK(cudaMemcpyAsync(d_lab, labels, n * sizeof(u64), cudaMemcpyHostToDevice, st));
-  CUDA_OK(cudaMemcpyAsync(d_ids, ids, 2 * nitems * sizeof(u64), cudaMemcpyHostToDevice, st));
-  CUDA_OK(cudaMemcpyAsync(d_probs, probs, n * nprob, cudaMemcpyHostToDevice, st));
-  CUDA_OK(cudaMemcpyAsync(d_table, mask_table, 256, cudaMemcpyHostToDevice, st));
-  CUDA_OK(cudaMemsetAsync(d_counts, 0, (size_t)nitems * ncounts * sizeof(u64), st));
-  std::vector<u64> counts((size_t)nitems * ncounts);
-  std::memset(stats_out, 0, (size_t)nitems * sizeof(FfnResegStats));
-
-  if (pair) {
-    // Four masks per item, then the exact squared EDT of every mask at once: with a single id, the nearest-id keys of
-    // decision_kernels.cuh are plain squared distances (M = 1).  Boxes are stacked along z for the x and y passes and
-    // seen as (masks, Z, Y * X) for the z pass, so that no line crosses a box.
-    const long long nmasks = 4 * nitems;
-    const size_t nk = (size_t)nmasks * nbox;
-    u64 *keys = nullptr, *keys2 = nullptr, *d_max = nullptr;
-    int *sbuf = nullptr, *tbuf = nullptr;
-    if (bufs.get(&keys, nk) || bufs.get(&keys2, nk) || bufs.get(&sbuf, nk) ||
-        bufs.get(&tbuf, nk) || bufs.get(&d_max, nmasks))
-      return 1;
-    CUDA_OK(cudaMemsetAsync(d_max, 0, nmasks * sizeof(u64), st));
-    rsk::pair_prepare<<<item_grid, 256, 0, st>>>(d_lab, d_probs, d_ids, d_table, nitems, nbox, keys, d_counts);
-    const int zs = (int)(nmasks * bz);
-    dpk::nid_x<<<blocks, 128, 0, st>>>(keys, zs, by, bx, (u64)w[2] * (u64)w[2], 1);
-    dpk::nid_line<<<blocks, 128, 0, st>>>(keys, keys2, 1, zs, by, bx, (u64)w[1] * (u64)w[1], sbuf, tbuf);
-    dpk::nid_line<<<blocks, 128, 0, st>>>(keys2, keys, 1, (int)nmasks, bz, by * bx, (u64)w[0] * (u64)w[0], sbuf, tbuf);
-    const dim3 mask_grid(item_grid.x, (unsigned)std::min<long long>(nmasks, 65535));
-    rsk::edt_max<<<mask_grid, 256, 0, st>>>(keys, nmasks, nbox, d_max);
-    CUDA_OK(cudaGetLastError());
-    std::vector<u64> maxes(nmasks);
-    CUDA_OK(cudaMemcpyAsync(maxes.data(), d_max, nmasks * sizeof(u64), cudaMemcpyDeviceToHost, st));
-    CUDA_OK(cudaMemcpyAsync(counts.data(), d_counts, counts.size() * sizeof(u64), cudaMemcpyDeviceToHost, st));
-    CUDA_OK(cudaStreamSynchronize(st));
-    // No voxel outside the mask: scipy's feature transform then points every voxel at (-1, 0, 0).
-    const u64 full = (u64)bz * bz * w[0] * w[0] + (u64)(by - 1) * (by - 1) * w[1] * w[1] +
-                     (u64)(bx - 1) * (bx - 1) * w[2] * w[2];
-    for (long long it = 0; it < nitems; ++it) {
-      const u64* c = &counts[it * rsk::kPairCounts];
-      FfnResegStats& s = stats_out[it];
-      s.n_seg[0] = (int64_t)c[0];
-      s.n_seg[1] = (int64_t)c[1];
-      s.n_reseg[0] = (int64_t)c[2];
-      s.n_reseg[1] = (int64_t)c[3];
-      s.n_reseg_seg[0][0] = (int64_t)c[4];
-      s.n_reseg_seg[0][1] = (int64_t)c[5];
-      s.n_reseg_seg[1][0] = (int64_t)c[6];
-      s.n_reseg_seg[1][1] = (int64_t)c[7];
-      s.n_inter = (int64_t)c[8];
-      s.n_union = (int64_t)c[9];
-      for (int k = 0; k < 4; ++k) s.max_edt2[k] = maxes[4 * it + k] == rsk::kInf ? full : maxes[4 * it + k];
-    }
-    return 0;
-  }
-
-  // Endpoint: |mask| per item, and the voxels of every (item, label) split by mask, by sorting on label and then
-  // (stably) on item.
-  if (nitems >= (1ll << 30)) return fail("too many endpoint items");
-  int ibits = 1;
-  while ((1ll << ibits) < nitems) ++ibits;
-  const int ni = (int)n;
-  int nruns = ni;   // an upper bound until the runs are counted: at most one row per voxel
-  u64* d_lab2 = nullptr;
-  unsigned *d_vals = nullptr, *d_vals2 = nullptr, *d_scan = nullptr;
-  unsigned char* d_head = nullptr;
-  int *d_heads = nullptr, *d_num = nullptr;
-  FfnResegOverlap *d_all = nullptr, *d_kept = nullptr;
-  if (bufs.get(&d_lab2, n) || bufs.get(&d_vals, n) || bufs.get(&d_vals2, n) || bufs.get(&d_scan, n) ||
-      bufs.get(&d_head, n) || bufs.get(&d_heads, n) || bufs.get(&d_num, 2))
-    return 1;
-  rsk::endpoint_prepare<<<item_grid, 256, 0, st>>>(d_lab, d_probs, d_ids, d_table, nitems, nbox, d_vals, d_counts);
-  auto sort_label = [&](void* t, size_t& b) {
-    return cub::DeviceRadixSort::SortPairs(t, b, d_lab, d_lab2, d_vals, d_vals2, ni, 0, 64, st);
-  };
-  auto sort_item = [&](void* t, size_t& b) {
-    return cub::DeviceRadixSort::SortPairs(t, b, d_vals2, d_vals, d_lab2, d_lab, ni, 1, 1 + ibits, st);
-  };
-  auto select_heads = [&](void* t, size_t& b) {
-    return cub::DeviceSelect::Flagged(t, b, cub::CountingInputIterator<int>(0), d_head, d_heads, d_num, ni, st);
-  };
-  auto scan = [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, d_vals2, d_scan, ni, st); };
-  auto select_rows = [&](void* t, size_t& b) {
-    return cub::DeviceSelect::If(t, b, d_all, d_kept, d_num + 1, nruns, rsk::Overlapping(), st);
-  };
-  CubTemp temp;
-  if (temp.alloc(bufs, sort_label, sort_item, select_heads, scan, select_rows)) return 1;
-  CUDA_OK(temp.run(sort_label));
-  CUDA_OK(temp.run(sort_item));
-  // Sorted by (item, label): d_vals = item << 1 | mask, d_lab = label.
-  rsk::run_heads<<<blocks, 256, 0, st>>>(d_vals, d_lab, ni, d_head, d_vals2);
-  CUDA_OK(temp.run(select_heads));
-  CUDA_OK(temp.run(scan));
-  CUDA_OK(cudaMemcpyAsync(&nruns, d_num, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaMemcpyAsync(counts.data(), d_counts, counts.size() * sizeof(u64), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  if (bufs.get(&d_all, nruns) || bufs.get(&d_kept, nruns)) return 1;
-  rsk::run_rows<<<blocks, 256, 0, st>>>(d_heads, nruns, ni, d_vals, d_lab, d_scan, d_all);
-  CUDA_OK(temp.run(select_rows));
-  CUDA_OK(cudaGetLastError());
-  int nkept = 0;
-  CUDA_OK(cudaMemcpyAsync(&nkept, d_num + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  const int64_t m = std::min<int64_t>(cap, nkept);
-  if (m > 0) CUDA_OK(cudaMemcpyAsync(overlaps_out, d_kept, m * sizeof(FfnResegOverlap), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  for (long long it = 0; it < nitems; ++it) {
-    stats_out[it].n_seg[0] = (int64_t)counts[2 * it];
-    stats_out[it].n_reseg[0] = (int64_t)counts[2 * it + 1];
-  }
-  *n_overlaps = nkept;
-  return 0;
-}
-
-namespace {
-struct MaxU64 {
-  __device__ __forceinline__ unsigned long long operator()(unsigned long long x, unsigned long long y) const {
-    return x > y ? x : y;
-  }
-};
-}  // namespace
-
-int ffn_split_intersection(int device, int64_t n, uint64_t* a, const uint64_t* b, int64_t min_size) {
-  using csk::u64;
-  if (n < 0 || (n > 0 && (!a || !b))) return fail("bad argument");
-  if (n >= (1ll << 31)) return fail("split consensus supports volumes of fewer than 2^31 voxels");
-  if (n == 0) return 0;
-  cudaDeviceProp prop{};
-  if (use_device(device, &prop)) return 1;
-  cudaStream_t st = cudaStreamPerThread;
-  const int blocks = prop.multiProcessorCount * 16;
-  const int ni = (int)n;
-  int np = ni;   // an upper bound until the (a, b) pairs are counted
-  DevBufs bufs;
-
-  u64 *d_a = nullptr, *d_b = nullptr, *d_tmp = nullptr, *d_max = nullptr;
-  int* d_num = nullptr;
-  if (bufs.get(&d_a, n) || bufs.get(&d_b, n) || bufs.get(&d_tmp, n) || bufs.get(&d_max, 2) || bufs.get(&d_num, 2))
-    return 1;
-  u64 *d_pairs = nullptr, *d_sw = nullptr, *d_sw2 = nullptr, *d_pack = nullptr, *d_best = nullptr, *d_lab = nullptr;
-  int *d_counts = nullptr, *d_idx = nullptr, *d_idx2 = nullptr, *d_flags = nullptr, *d_rank = nullptr;
-  unsigned *d_aof = nullptr, *d_ured = nullptr;
-  unsigned char* d_partner = nullptr;
-  // The CUB calls (max_of, sort_keys and unique run on several arrays), sized for n items: no later call has more.
-  auto max_of = [&](u64* in, u64* out) {
-    return [=](void* t, size_t& b) { return cub::DeviceReduce::Max(t, b, in, out, ni, st); };
-  };
-  auto sort_keys = [&](u64* in, u64* out) {
-    return [=](void* t, size_t& b) { return cub::DeviceRadixSort::SortKeys(t, b, in, out, ni, 0, 64, st); };
-  };
-  auto unique = [&](u64* out) {
-    return [=](void* t, size_t& b) { return cub::DeviceSelect::Unique(t, b, d_tmp, out, d_num, ni, st); };
-  };
-  auto rle = [&](void* t, size_t& b) {
-    return cub::DeviceRunLengthEncode::Encode(t, b, d_b, d_pairs, d_counts, d_num, ni, st);
-  };
-  auto sort_pairs = [&](void* t, size_t& b) {
-    return cub::DeviceRadixSort::SortPairs(t, b, d_sw, d_sw2, d_idx, d_idx2, np, 0, 64, st);
-  };
-  auto reduce_best = [&](void* t, size_t& b) {
-    return cub::DeviceReduce::ReduceByKey(t, b, d_aof, d_ured, d_pack, d_best, d_num + 1, MaxU64(), np, st);
-  };
-  auto scan = [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_flags, d_rank, np, st); };
-  CubTemp temp;
-  if (temp.alloc(bufs, max_of(d_a, d_max), sort_keys(d_a, d_tmp), unique(d_a), rle, sort_pairs, reduce_best, scan))
-    return 1;
-  CUDA_OK(cudaMemcpyAsync(d_a, a, n * sizeof(u64), cudaMemcpyHostToDevice, st));
-  CUDA_OK(cudaMemcpyAsync(d_b, b, n * sizeof(u64), cudaMemcpyHostToDevice, st));
-  CUDA_OK(temp.run(max_of(d_a, d_max)));
-  CUDA_OK(temp.run(max_of(d_b, d_max + 1)));
-  u64 maxes[2] = {0, 0};
-  CUDA_OK(cudaMemcpyAsync(maxes, d_max, sizeof(maxes), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  const u64 max_id = maxes[0];
-
-  // remap_input: sorted unique ids of an array whose ids do not fit in 32 bits, and the +1 shift when 0 is absent.
-  u64* uniq[2] = {nullptr, nullptr};
-  int nuniq[2] = {0, 0};
-  unsigned shift[2] = {0, 0};
-  for (int k = 0; k < 2; ++k) {
-    if (maxes[k] <= 0xffffffffull) continue;
-    CUDA_OK(temp.run(sort_keys(k ? d_b : d_a, d_tmp)));
-    if (bufs.get(&uniq[k], n)) return 1;
-    CUDA_OK(temp.run(unique(uniq[k])));
-    u64 first = 0;
-    CUDA_OK(cudaMemcpyAsync(&nuniq[k], d_num, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CUDA_OK(cudaMemcpyAsync(&first, uniq[k], sizeof(u64), cudaMemcpyDeviceToHost, st));
-    CUDA_OK(cudaStreamSynchronize(st));
-    shift[k] = first != 0;
-  }
-
-  // Joint keys (kept in d_tmp for the relabel), sorted into d_b, then the unique pairs and their counts.
-  csk::joint_keys<<<blocks, 256, 0, st>>>(d_a, d_b, (size_t)n, uniq[0], nuniq[0], shift[0], uniq[1], nuniq[1],
-                                          shift[1], d_tmp);
-  CUDA_OK(cudaGetLastError());
-  if (uniq[1]) bufs.release(uniq[1]);
-  CUDA_OK(temp.run(sort_keys(d_tmp, d_b)));
-  if (bufs.get(&d_pairs, n) || bufs.get(&d_counts, n)) return 1;
-  CUDA_OK(temp.run(rle));
-  CUDA_OK(cudaMemcpyAsync(&np, d_num, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  bufs.release(d_b);
-
-  // Largest overlap per a: the pairs regrouped by a (a-major sort), then a maximum of count << 32 | ~b per a.
-  if (bufs.get(&d_sw, np) || bufs.get(&d_sw2, np) || bufs.get(&d_pack, np) || bufs.get(&d_best, np) ||
-      bufs.get(&d_lab, np) || bufs.get(&d_idx, np) || bufs.get(&d_idx2, np) || bufs.get(&d_flags, np) ||
-      bufs.get(&d_rank, np) || bufs.get(&d_aof, np) || bufs.get(&d_ured, np) || bufs.get(&d_partner, np))
-    return 1;
-  csk::regroup<<<blocks, 256, 0, st>>>(d_pairs, np, d_sw, d_idx);
-  CUDA_OK(temp.run(sort_pairs));
-  csk::partner_pack<<<blocks, 256, 0, st>>>(d_sw2, d_idx2, d_counts, np, d_aof, d_pack);
-  CUDA_OK(temp.run(reduce_best));
-  int nu = 0;
-  CUDA_OK(cudaMemcpyAsync(&nu, d_num + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  csk::mark_partner<<<blocks, 256, 0, st>>>(d_aof, d_pack, d_idx2, d_ured, d_best, nu, np, d_partner);
-
-  // New ids in key order, then the output id of every pair.
-  csk::pair_flags<<<blocks, 256, 0, st>>>(d_pairs, d_counts, d_partner, np, (long long)min_size, d_flags);
-  CUDA_OK(temp.run(scan));
-  int last[2] = {0, 0};
-  CUDA_OK(cudaMemcpyAsync(&last[0], d_flags + np - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaMemcpyAsync(&last[1], d_rank + np - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  const u64 n_new = (u64)last[0] + (u64)last[1];
-  if (n_new > ~0ull - max_id)
-    return fail("split consensus: max id " + std::to_string(max_id) + " + " + std::to_string(n_new) +
-                " new ids does not fit in 64 bits");
-  csk::pair_labels<<<blocks, 256, 0, st>>>(d_pairs, d_counts, d_partner, d_rank, np, (long long)min_size, uniq[0],
-                                           shift[0], max_id, d_lab);
-  csk::relabel<<<blocks, 256, 0, st>>>(d_tmp, (size_t)n, d_pairs, np, d_lab, d_a);
-  CUDA_OK(cudaGetLastError());
-  CUDA_OK(cudaMemcpyAsync(a, d_a, n * sizeof(u64), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  return 0;
-}
-
-int ffn_compute_partitions(int device, const FfnPartitionDesc* desc, uint64_t* labels, const uint8_t* mask,
-                           uint8_t* out, int64_t counts[256]) {
-  using ptk::u64;
-  if (!desc || !labels || !out || !counts || desc->n_thresholds < 0 || (desc->n_thresholds > 0 && !desc->thresholds) ||
-      desc->n_spheres < 0 || (desc->n_spheres > 0 && !desc->spheres) || desc->n_whitelist < 0 ||
-      (desc->n_whitelist > 0 && !desc->whitelist))
-    return fail("bad argument");
-  ptk::Geometry g{};
-  size_t n = 1, nout = 1;
-  for (int a = 0; a < 3; ++a) {
-    g.s[a] = desc->shape_zyx[a];
-    g.r[a] = desc->lom_radius_zyx[a];
-    if (g.s[a] < 0) return fail("shape must not be negative");
-    if (g.r[a] < 0) return fail("the LOM radius must not be negative");
-    g.o[a] = (int)std::max<int64_t>((int64_t)g.s[a] - 2 * (int64_t)g.r[a], 0);
-    n *= (size_t)g.s[a];
-    nout *= (size_t)g.o[a];
-  }
-  if (n >= (1ull << 31)) return fail("partition maps support volumes of fewer than 2^31 voxels");
-  std::fill(counts, counts + 256, (int64_t)0);
-  if (desc->n_labels_out) *desc->n_labels_out = 0;
-  if (n == 0) return 0;
-  cudaDeviceProp prop{};
-  if (use_device(device, &prop)) return 1;
-  cudaStream_t st = cudaStreamPerThread;
-  const int blocks = prop.multiProcessorCount * 16;
-  const int ni = (int)n;
-  DevBufs bufs;
-
-  // Compaction: sorted unique ids and their counts.
-  u64 *d_lab = nullptr, *d_sorted = nullptr, *d_unique = nullptr;
-  unsigned* d_cnt = nullptr;
-  int* d_num = nullptr;
-  if (bufs.get(&d_lab, n) || bufs.get(&d_sorted, n) || bufs.get(&d_unique, n) || bufs.get(&d_cnt, n) ||
-      bufs.get(&d_num, 1))
-    return 1;
-  auto sort = [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortKeys(t, b, d_lab, d_sorted, ni, 0, 64, st); };
-  auto rle = [&](void* t, size_t& b) {
-    return cub::DeviceRunLengthEncode::Encode(t, b, d_sorted, d_unique, d_cnt, d_num, ni, st);
-  };
-  CubTemp temp;
-  if (temp.alloc(bufs, sort, rle)) return 1;
-  CUDA_OK(cudaMemcpyAsync(d_lab, labels, n * sizeof(u64), cudaMemcpyHostToDevice, st));
-  CUDA_OK(temp.run(sort));
-  CUDA_OK(temp.run(rle));
-  int nruns = 0;
-  CUDA_OK(cudaMemcpyAsync(&nruns, d_num, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  std::vector<u64> ids(nruns);
-  std::vector<unsigned> sizes(nruns);
-  CUDA_OK(cudaMemcpyAsync(ids.data(), d_unique, nruns * sizeof(u64), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaMemcpyAsync(sizes.data(), d_cnt, nruns * sizeof(unsigned), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  bufs.release(d_sorted);
-  bufs.release(d_cnt);
-  bufs.release(temp.p);
-
-  // Run codes: dust (cleared), skipped (0, or outside the whitelist) or the compact id, in uint64 id order.
-  std::vector<u64> white(desc->whitelist, desc->whitelist + desc->n_whitelist);
-  std::sort(white.begin(), white.end());
-  std::vector<int> code(nruns);
-  int nk = 0;
-  bool dust = false;
-  for (int i = 0; i < nruns; ++i) {
-    if (ids[i] != 0 && desc->min_size > 0 && (int64_t)sizes[i] < desc->min_size) {
-      code[i] = ptk::kDust;
-      dust = true;
-    } else if (ids[i] == 0 || (desc->use_whitelist && !std::binary_search(white.begin(), white.end(), ids[i]))) {
-      code[i] = ptk::kSkipped;
-    } else {
-      code[i] = nk++;
-    }
-  }
-  if (desc->n_labels_out) *desc->n_labels_out = nk;
-  int *d_code = nullptr, *d_compact = nullptr, *d_bmin = nullptr, *d_bmax = nullptr;
-  if (bufs.get(&d_code, nruns) || bufs.get(&d_compact, n) || bufs.get(&d_bmin, 3 * (size_t)nk) ||
-      bufs.get(&d_bmax, 3 * (size_t)nk))
-    return 1;
-  CUDA_OK(cudaMemcpyAsync(d_code, code.data(), nruns * sizeof(int), cudaMemcpyHostToDevice, st));
-  CUDA_OK(cudaMemsetAsync(d_bmin, 0x7f, 3 * (size_t)nk * sizeof(int), st));
-  CUDA_OK(cudaMemsetAsync(d_bmax, 0xff, 3 * (size_t)nk * sizeof(int), st));
-  ptk::compact_ids<<<blocks, 256, 0, st>>>(d_lab, n, d_unique, nruns, d_code, d_compact, d_bmin, d_bmax, g.s[1], g.s[2]);
-  CUDA_OK(cudaGetLastError());
-  if (dust) CUDA_OK(cudaMemcpyAsync(labels, d_lab, n * sizeof(u64), cudaMemcpyDeviceToHost, st));
-  std::vector<int> bmin(3 * (size_t)nk), bmax(3 * (size_t)nk);
-  if (nk > 0) {
-    CUDA_OK(cudaMemcpyAsync(bmin.data(), d_bmin, bmin.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
-    CUDA_OK(cudaMemcpyAsync(bmax.data(), d_bmax, bmax.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
-  }
-  CUDA_OK(cudaStreamSynchronize(st));
-  bufs.release(d_lab);
-  bufs.release(d_unique);
-  bufs.release(d_code);
-  if (nout == 0) {
-    CUDA_OK(cudaGetLastError());
-    return 0;
-  }
-
-  unsigned char* d_out = nullptr;
-  if (bufs.get(&d_out, nout)) return 1;
-  CUDA_OK(cudaMemsetAsync(d_out, 0, nout, st));
-
-  // Grown boxes: the windows of a label's voxels inside the VALID region, i.e. its box clipped to [r, s - r) and
-  // grown by r.  A label with no voxel there writes nothing and is left out.
-  std::vector<ptk::LabelBox> boxes;
-  std::vector<long long> vols;
-  for (int k = 0; k < nk; ++k) {
-    ptk::LabelBox b{};
-    b.k = k;
-    bool empty = false;
-    for (int a = 0; a < 3; ++a) {
-      const int lo = std::max(bmin[3 * k + a], g.r[a]), hi = std::min(bmax[3 * k + a] + 1, g.s[a] - g.r[a]);
-      empty |= lo >= hi;
-      b.lo[a] = lo - g.r[a];
-      b.n[a] = hi - lo + 2 * g.r[a];
-    }
-    if (empty) continue;
-    boxes.push_back(b);
-    vols.push_back((long long)b.n[0] * b.n[1] * b.n[2]);
-  }
-  // Groups whose two int32 scratch arrays fit the budget, in label order.
-  long long budget = desc->scratch_bytes;
-  if (budget <= 0) {
-    size_t free_b = 0, total_b = 0;
-    CUDA_OK(cudaMemGetInfo(&free_b, &total_b));
-    budget = (long long)(free_b / 4);
-  }
-  const long long per_vox = 2 * (long long)sizeof(int);
-  std::vector<size_t> group_start{0};
-  long long gvol = 0, max_gvol = 0;
-  for (size_t j = 0; j < boxes.size(); ++j) {
-    if (j > group_start.back() && (gvol + vols[j]) * per_vox > budget) {
-      group_start.push_back(j);
-      gvol = 0;
-    }
-    ptk::LabelBox& b = boxes[j];
-    if (j > group_start.back()) {   // the first box of a group starts at scratch voxel 0 and line 0
-      const ptk::LabelBox& p = boxes[j - 1];
-      b.off = p.off + vols[j - 1];
-      b.line[0] = p.line[0] + (long long)p.n[0] * p.n[1];
-      b.line[1] = p.line[1] + (long long)p.n[0] * p.n[2];
-      b.line[2] = p.line[2] + (long long)p.n[1] * p.n[2];
-    }
-    gvol += vols[j];
-    max_gvol = std::max(max_gvol, gvol);
-  }
-  group_start.push_back(boxes.size());
-
-  if (!boxes.empty()) {
-    ptk::LabelBox* d_boxes = nullptr;
-    double* d_th = nullptr;
-    int *d_A = nullptr, *d_B = nullptr;
-    if (bufs.get(&d_boxes, boxes.size()) || bufs.get(&d_th, desc->n_thresholds) || bufs.get(&d_A, max_gvol) ||
-        bufs.get(&d_B, max_gvol))
-      return 1;
-    CUDA_OK(cudaMemcpyAsync(d_boxes, boxes.data(), boxes.size() * sizeof(ptk::LabelBox), cudaMemcpyHostToDevice, st));
-    if (desc->n_thresholds)
-      CUDA_OK(cudaMemcpyAsync(d_th, desc->thresholds, desc->n_thresholds * sizeof(double), cudaMemcpyHostToDevice, st));
-    const double fov = (double)(2 * g.r[0] + 1) * (double)(2 * g.r[1] + 1) * (double)(2 * g.r[2] + 1);
-    auto grid_for = [&](long long lines) { return (int)std::min<long long>((lines + 255) / 256, blocks * 2); };
-    for (size_t gi = 0; gi + 1 < group_start.size(); ++gi) {
-      const size_t j0 = group_start[gi], j1 = group_start[gi + 1];
-      const ptk::LabelBox& last = boxes[j1 - 1];
-      const int nb = (int)(j1 - j0);
-      const long long lx = last.line[0] + (long long)last.n[0] * last.n[1];
-      const long long ly = last.line[1] + (long long)last.n[0] * last.n[2];
-      const long long lz = last.line[2] + (long long)last.n[1] * last.n[2];
-      ptk::count_x<<<grid_for(lx), 256, 0, st>>>(d_compact, d_boxes + j0, nb, lx, g, d_A);
-      ptk::count_y<<<grid_for(ly), 256, 0, st>>>(d_A, d_boxes + j0, nb, ly, g, d_B);
-      ptk::count_z<<<grid_for(lz), 256, 0, st>>>(d_B, d_compact, d_boxes + j0, nb, lz, g, fov, d_th,
-                                                  desc->n_thresholds, d_out);
-      CUDA_OK(cudaGetLastError());
-    }
-    CUDA_OK(cudaStreamSynchronize(st));
-    bufs.release(d_A);
-    bufs.release(d_B);
-  }
-  bufs.release(d_compact);
-
-  // Mask: any() over the LOM box, one axis at a time (x, then y, then z).
-  unsigned char* d_masked = nullptr;
-  if (mask) {
-    unsigned char *d_m0 = nullptr, *d_m1 = nullptr;
-    if (bufs.get(&d_m0, n) || bufs.get(&d_m1, n)) return 1;
-    CUDA_OK(cudaMemcpyAsync(d_m0, mask, n, cudaMemcpyHostToDevice, st));
-    ptk::box_any<<<blocks, 256, 0, st>>>(d_m0, d_m1, 2, g.r[2], g.s[0], g.s[1], g.s[2]);
-    ptk::box_any<<<blocks, 256, 0, st>>>(d_m1, d_m0, 1, g.r[1], g.s[0], g.s[1], g.o[2]);
-    ptk::box_any<<<blocks, 256, 0, st>>>(d_m0, d_m1, 0, g.r[0], g.s[0], g.o[1], g.o[2]);
-    CUDA_OK(cudaGetLastError());
-    d_masked = d_m1;
-  }
-  ptk::Sphere* d_sph = nullptr;
-  unsigned long long* d_hist = nullptr;
-  if (bufs.get(&d_sph, desc->n_spheres) || bufs.get(&d_hist, 256)) return 1;
-  std::vector<ptk::Sphere> sph(desc->n_spheres);
-  for (int s = 0; s < desc->n_spheres; ++s) {
-    const FfnExclusionSphere& e = desc->spheres[s];
-    for (int a = 0; a < 3; ++a) {
-      sph[s].c[a] = e.c_xyz[a];
-      sph[s].fc[a] = e.f_xyz[a];
-    }
-    sph[s].r2 = e.r2;
-    sph[s].fr2 = e.f_r2;
-    sph[s].integer = e.integer;
-  }
-  if (!sph.empty())
-    CUDA_OK(cudaMemcpyAsync(d_sph, sph.data(), sph.size() * sizeof(ptk::Sphere), cudaMemcpyHostToDevice, st));
-  CUDA_OK(cudaMemsetAsync(d_hist, 0, 256 * sizeof(unsigned long long), st));
-  ptk::finish<<<blocks, 256, 0, st>>>(d_out, nout, d_masked, d_sph, desc->n_spheres, g, d_hist);
-  CUDA_OK(cudaGetLastError());
-  CUDA_OK(cudaMemcpyAsync(out, d_out, nout, cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaMemcpyAsync(counts, d_hist, 256 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  CUDA_OK(cudaGetLastError());
-  return 0;
-}
-
-int ffn_partition_rows(int device, const FfnPartitionRowsDesc* desc, const uint8_t* volume, int64_t* rows,
-                       int64_t counts[256]) {
-  if (!desc || !volume || !rows || !counts) return fail("bad argument");
-  cok::Crop c{};
-  size_t nvol = 1;
-  long long ncrop = 1;
-  for (int a = 0; a < 3; ++a) {
-    const int s = desc->shape_zyx[a], lo = desc->crop_start_zyx[a], n = desc->crop_shape_zyx[a];
-    if (s < 0 || lo < 0 || n < 0 || (int64_t)lo + n > s) return fail("the crop must lie inside the volume");
-    c.n[a] = n;
-    c.lo[a] = lo;
-    nvol *= (size_t)s;
-    ncrop *= n;
-  }
-  if (ncrop >= (1ll << 31)) return fail("partition crops must have fewer than 2^31 voxels");
-  c.sy = desc->shape_zyx[2];
-  c.sz = (long long)desc->shape_zyx[1] * desc->shape_zyx[2];
-  c.size = ncrop;
-  std::fill(counts, counts + 256, (int64_t)0);
-  if (ncrop == 0) return 0;
-  cudaDeviceProp prop{};
-  if (use_device(device, &prop)) return 1;
-  cudaStream_t st = cudaStreamPerThread;
-  const int ntiles = (int)((ncrop + cok::kTile - 1) / cok::kTile);
-  const size_t nhist = (size_t)256 * ntiles;
-  DevBufs bufs;
-  unsigned char* d_vol = nullptr;
-  int *d_hist = nullptr, *d_base = nullptr;
-  unsigned long long* d_counts = nullptr;
-  longlong2* d_rows = nullptr;
-  auto scan = [&](void* t, size_t& b) {
-    return cub::DeviceScan::ExclusiveSum(t, b, d_hist, d_base, (int64_t)nhist, st);
-  };
-  CubTemp temp;
-  if (bufs.get(&d_vol, nvol) || bufs.get(&d_hist, nhist) || bufs.get(&d_base, nhist) || bufs.get(&d_counts, 256) ||
-      temp.alloc(bufs, scan))
-    return 1;
-  CUDA_OK(cudaMemcpyAsync(d_vol, volume, nvol, cudaMemcpyHostToDevice, st));
-  CUDA_OK(cudaMemsetAsync(d_counts, 0, 256 * sizeof(unsigned long long), st));
-  cok::bucket_hist<<<ntiles, cok::kThreads, 0, st>>>(d_vol, c, ntiles, d_hist, d_counts);
-  CUDA_OK(cudaGetLastError());
-  CUDA_OK(temp.run(scan));
-  CUDA_OK(cudaMemcpyAsync(counts, d_counts, 256 * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  bufs.release(d_hist);
-  bufs.release(temp.p);
-  const long long kept = ncrop - counts[cok::kIgnore];
-  if (bufs.get(&d_rows, kept)) return 1;
-  cok::bucket_scatter<<<ntiles, cok::kThreads, 0, st>>>(d_vol, c, ntiles, d_base, desc->volume_index, d_rows);
-  CUDA_OK(cudaGetLastError());
-  if (kept > 0)
-    CUDA_OK(cudaMemcpyAsync(rows, d_rows, kept * sizeof(longlong2), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  CUDA_OK(cudaGetLastError());
-  return 0;
-}
-
-int ffn_coordinate_records(int device, const FfnCoordinateDesc* desc, const int64_t* rows, int64_t n_rows,
-                           uint8_t* out, int64_t out_capacity, int64_t* out_bytes) {
-  if (!desc || !out_bytes || n_rows < 0 || (n_rows > 0 && (!rows || !out)) || desc->n_volumes < 0 ||
-      (desc->n_volumes > 0 && !desc->volumes) || desc->names_bytes < 0 || (desc->names_bytes > 0 && !desc->names))
-    return fail("bad argument");
-  if (n_rows >= (1ll << 38)) return fail("too many rows in one call");
-  std::vector<cok::Volume> vols(desc->n_volumes);
-  for (int i = 0; i < desc->n_volumes; ++i) {
-    const FfnCoordinateVolume& v = desc->volumes[i];
-    for (int a = 0; a < 3; ++a) {
-      if (v.crop_shape_zyx[a] < 0 || v.margin_zyx[a] < 0 || (int64_t)v.margin_zyx[a] + v.crop_shape_zyx[a] >= (1ll << 31))
-        return fail("crop shapes and margins must be non-negative and their sum below 2^31");
-      vols[i].n[a] = v.crop_shape_zyx[a];
-      vols[i].margin[a] = v.margin_zyx[a];
-    }
-    if (v.name_offset < 0 || v.name_length < 0 || v.name_offset > desc->names_bytes ||
-        v.name_length > desc->names_bytes - v.name_offset)
-      return fail("a volume name lies outside the names");
-    vols[i].name_off = v.name_offset;
-    vols[i].name_len = v.name_length;
-  }
-  *out_bytes = 0;
-  if (n_rows == 0) return 0;
-  cudaDeviceProp prop{};
-  if (use_device(device, &prop)) return 1;
-  cudaStream_t st = cudaStreamPerThread;
-  const long long nblocks = (n_rows + cok::kThreads - 1) / cok::kThreads;
-  DevBufs bufs;
-  longlong2* d_rows = nullptr;
-  cok::Volume* d_vols = nullptr;
-  unsigned char *d_names = nullptr, *d_out = nullptr;
-  cok::u64 *d_sums = nullptr, *d_offs = nullptr;
-  int* d_bad = nullptr;
-  auto scan = [&](void* t, size_t& b) {
-    return cub::DeviceScan::ExclusiveSum(t, b, d_sums, d_offs, (int64_t)nblocks + 1, st);
-  };
-  CubTemp temp;
-  if (bufs.get(&d_rows, n_rows) || bufs.get(&d_vols, vols.size()) || bufs.get(&d_names, desc->names_bytes) ||
-      bufs.get(&d_sums, nblocks + 1) || bufs.get(&d_offs, nblocks + 1) || bufs.get(&d_bad, 1) || temp.alloc(bufs, scan))
-    return 1;
-  CUDA_OK(cudaMemcpyAsync(d_rows, rows, n_rows * sizeof(longlong2), cudaMemcpyHostToDevice, st));
-  if (!vols.empty())
-    CUDA_OK(cudaMemcpyAsync(d_vols, vols.data(), vols.size() * sizeof(cok::Volume), cudaMemcpyHostToDevice, st));
-  if (desc->names_bytes)
-    CUDA_OK(cudaMemcpyAsync(d_names, desc->names, desc->names_bytes, cudaMemcpyHostToDevice, st));
-  CUDA_OK(cudaMemsetAsync(d_sums + nblocks, 0, sizeof(cok::u64), st));
-  CUDA_OK(cudaMemsetAsync(d_bad, 0, sizeof(int), st));
-  cok::record_sums<<<(unsigned)nblocks, cok::kThreads, 0, st>>>(d_rows, n_rows, d_vols, desc->n_volumes, d_sums, d_bad);
-  CUDA_OK(cudaGetLastError());
-  CUDA_OK(temp.run(scan));
-  cok::u64 total = 0;
-  int bad = 0;
-  CUDA_OK(cudaMemcpyAsync(&total, d_offs + nblocks, sizeof(total), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaMemcpyAsync(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  if (bad) return fail("a row's volume or flat index lies outside the volume table");
-  *out_bytes = (int64_t)total;
-  if ((int64_t)total > out_capacity) return fail("the output buffer is smaller than the records");
-  if (bufs.get(&d_out, total)) return 1;
-  cok::write_records<<<(unsigned)nblocks, cok::kThreads, 0, st>>>(d_rows, n_rows, d_vols, desc->n_volumes, d_names,
-                                                                  d_offs, d_out);
-  CUDA_OK(cudaGetLastError());
-  CUDA_OK(cudaMemcpyAsync(out, d_out, total, cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  CUDA_OK(cudaGetLastError());
-  return 0;
-}
-
-int ffn_clean_up(int device, const FfnCleanUpDesc* desc, uint64_t* labels, uint64_t* ids, uint64_t* orig_ids,
-                 int64_t* counts, int64_t cap, int64_t* n_ids) {
-  using cck::u64;
-  const bool table = ids || orig_ids || counts;
-  if (!desc || !n_ids || cap < 0 || (cap > 0 && !table)) return fail("bad argument");
-  const int sz = desc->shape_zyx[0], sy = desc->shape_zyx[1], sx = desc->shape_zyx[2];
-  if (sz < 0 || sy < 0 || sx < 0) return fail("shape must not be negative");
-  if (desc->connectivity < 1 || desc->connectivity > 3) return fail("connectivity must be 1, 2 or 3");
-  // Every extent is below 2^31, and sz * sy is checked before it is multiplied by sx, so no product wraps.
-  size_t n = 0;
-  if (sz && sy && sx) {
-    if ((size_t)sz * sy >= (1ull << 31) || (size_t)sz * sy * sx >= (1ull << 31))
-      return fail("connected components support volumes of fewer than 2^31 voxels");
-    n = (size_t)sz * sy * sx;
-  }
-  *n_ids = 0;
-  if (n == 0) return 0;
-  if (!labels) return fail("bad argument");
-  cudaDeviceProp prop{};
-  if (use_device(device, &prop)) return 1;
-  cudaStream_t st = cudaStreamPerThread;
-  const int blocks = prop.multiProcessorCount * 16;
-  const int ni = (int)n;
-  const long long min_size = desc->min_size;
-  DevBufs bufs;
-
-  u64 *d_lab = nullptr, *d_out = nullptr;
-  int *d_par = nullptr, *d_cnt = nullptr, *d_rank = nullptr, *d_roots = nullptr, *d_misc = nullptr;
-  // d_misc: [0] first output zero, [1] output zeros, [2] kept components
-  if (bufs.get(&d_lab, n) || bufs.get(&d_out, n) || bufs.get(&d_par, n) || bufs.get(&d_cnt, n, true) ||
-      bufs.get(&d_rank, n) || bufs.get(&d_misc, 3, true) || (table && bufs.get(&d_roots, n)))
-    return 1;
-  cub::CountingInputIterator<int> index(0);
-  cub::TransformInputIterator<int, cck::IsRoot, cub::CountingInputIterator<int>> is_root(index, cck::IsRoot{d_par});
-  auto scan = [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, is_root, d_rank, ni, st); };
-  auto select = [&](void* t, size_t& b) {
-    return cub::DeviceSelect::If(t, b, index, d_roots, d_misc + 2, ni, cck::KeptRoot{d_par, d_cnt, min_size}, st);
-  };
-  CubTemp temp;
-  if (table ? temp.alloc(bufs, scan, select) : temp.alloc(bufs, scan)) return 1;
-  CUDA_OK(cudaMemcpyAsync(d_lab, labels, n * sizeof(u64), cudaMemcpyHostToDevice, st));
-  const cck::Shape shape{sz, sy, sx};
-  cck::init<<<blocks, cck::kBlock, 0, st>>>(d_lab, ni, sx, d_par, d_misc);
-  switch (desc->connectivity) {
-    case 1: cck::merge<1><<<blocks, cck::kBlock, 0, st>>>(d_lab, shape, d_par); break;
-    case 2: cck::merge<2><<<blocks, cck::kBlock, 0, st>>>(d_lab, shape, d_par); break;
-    default: cck::merge<3><<<blocks, cck::kBlock, 0, st>>>(d_lab, shape, d_par); break;
-  }
-  cck::flatten_count<<<blocks, cck::kBlock, 0, st>>>(d_par, ni, d_cnt);
-  CUDA_OK(cudaGetLastError());
-  CUDA_OK(temp.run(scan));
-  cck::write_labels<<<blocks, cck::kBlock, 0, st>>>(d_par, d_rank, d_cnt, ni, min_size, d_out, d_misc, d_misc + 1);
-  CUDA_OK(cudaGetLastError());
-  if (table) CUDA_OK(temp.run(select));
-  int misc[3] = {0, 0, 0};
-  CUDA_OK(cudaMemcpyAsync(misc, d_misc, sizeof(misc), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  const int first_zero = misc[1] > 0 ? misc[0] : -1;
-
-  // The table: the 0 row first when the output has a 0, then the kept components in id order.  A table larger than
-  // cap leaves everything unwritten, so the caller can repeat the call on the same input with cap = *n_ids.
-  if (table) {
-    const int nkept = misc[2];
-    const int z = first_zero >= 0;
-    *n_ids = (int64_t)nkept + z;
-    if (*n_ids > cap) return 0;
-    u64 *d_ids = nullptr, *d_orig = nullptr;
-    long long* d_counts = nullptr;
-    if (bufs.get(&d_ids, nkept) || bufs.get(&d_orig, nkept) || bufs.get(&d_counts, nkept)) return 1;
-    cck::gather_rows<<<blocks, cck::kBlock, 0, st>>>(d_roots, nkept, d_rank, d_cnt, d_lab, d_ids, d_orig, d_counts);
-    CUDA_OK(cudaGetLastError());
-    if (ids && nkept) CUDA_OK(cudaMemcpyAsync(ids + z, d_ids, nkept * sizeof(u64), cudaMemcpyDeviceToHost, st));
-    if (orig_ids && nkept) CUDA_OK(cudaMemcpyAsync(orig_ids + z, d_orig, nkept * sizeof(u64), cudaMemcpyDeviceToHost, st));
-    if (counts && nkept) CUDA_OK(cudaMemcpyAsync(counts + z, d_counts, nkept * sizeof(long long), cudaMemcpyDeviceToHost, st));
-    if (z) {
-      if (ids) ids[0] = 0;
-      if (orig_ids) orig_ids[0] = labels[first_zero];   // labels still holds the input
-      if (counts) counts[0] = misc[1];
-    }
-  }
-  CUDA_OK(cudaMemcpyAsync(labels, d_out, n * sizeof(u64), cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  return 0;
-}
-
-// D = A * B^T through selftest::wgmma_kat_kernel on small-integer operands, exact in fp32: out[0..2] are the worst
-// errors with A shifted by 0, 3 and 35 rows (0 expected), out[3] the one with LBO and SBO swapped (large expected), and
-// the other slots -1.
-int ffn_selftest_wgmma(int device, double* out, int n_out) {
-  if (!out || n_out < 8) return fail("need >= 8 output slots");
-  cudaDeviceProp prop{};
-  if (use_device(device, &prop)) return 1;
-  for (int i = 0; i < n_out; ++i) out[i] = -1.0;
-  const int K = 64, kch = K / 8, rows_total = 256;   // A window has room for shifts up to 127 rows
-  std::vector<float> a((size_t)rows_total * K), b((size_t)96 * K);
-  unsigned s = 12345u;
-  auto rnd = [&]() {
-    s = s * 1664525u + 1013904223u;
-    return (float)((int)((s >> 20) & 15) - 8) * 0.125f;
-  };
-  for (auto& v : a) v = rnd();
-  for (auto& v : b) v = rnd();
-  std::vector<__half> ah((size_t)kch * rows_total * 8), bh((size_t)kch * 96 * 8);
-  for (int r = 0; r < rows_total; ++r)
-    for (int k = 0; k < K; ++k) ah[((size_t)(k / 8) * rows_total + r) * 8 + k % 8] = __float2half_rn(a[(size_t)r * K + k]);
-  for (int n = 0; n < 96; ++n)
-    for (int k = 0; k < K; ++k)
-      bh[(((size_t)(k / 8)) * 12 + n / 8) * 64 + (n % 8) * 8 + k % 8] = __float2half_rn(b[(size_t)n * K + k]);
-  DevBufs bufs;
-  __half *d_a = nullptr, *d_b = nullptr;
-  float* d_d = nullptr;
-  if (bufs.get(&d_a, ah.size()) || bufs.get(&d_b, bh.size()) || bufs.get(&d_d, 128 * 96)) return 1;
-  CUDA_OK(cudaMemcpy(d_a, ah.data(), ah.size() * 2, cudaMemcpyHostToDevice));
-  CUDA_OK(cudaMemcpy(d_b, bh.data(), bh.size() * 2, cudaMemcpyHostToDevice));
-  // the swapped-descriptor case strides 8-row groups by a_lbo / b_lbo and reaches ~58 KB past the operand base:
-  // allocate that much so the wrong answer is a wrong number, not an out-of-range shared-memory read
-  const int smem = 64 * 1024;
-  CUDA_OK(cudaFuncSetAttribute(selftest::wgmma_kat_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  const uint32_t a_lbo = rows_total * 16, a_sbo = 128, b_lbo = 12 * 128, b_sbo = 128;
-  struct Case { int shift; bool swapped; };
-  const Case cases[4] = {{0, false}, {3, false}, {35, false}, {0, true}};
-  for (int ci = 0; ci < 4; ++ci) {
-    const Case& c = cases[ci];
-    CUDA_OK(cudaMemset(d_d, 0xff, 128 * 96 * 4));
-    selftest::wgmma_kat_kernel<<<1, 256, smem>>>(d_a, rows_total, d_b, kch, c.shift, c.swapped ? a_sbo : a_lbo,
-                                                 c.swapped ? a_lbo : a_sbo, c.swapped ? b_sbo : b_lbo,
-                                                 c.swapped ? b_lbo : b_sbo, d_d);
-    CUDA_OK(cudaGetLastError());
-    CUDA_OK(cudaDeviceSynchronize());
-    std::vector<float> d(128 * 96);
-    CUDA_OK(cudaMemcpy(d.data(), d_d, d.size() * 4, cudaMemcpyDeviceToHost));
-    double worst = 0;
-    for (int r = 0; r < 128; ++r)
-      for (int n = 0; n < 96; ++n) {
-        double ref = 0;
-        for (int k = 0; k < K; ++k) ref += (double)a[(size_t)(r + c.shift) * K + k] * (double)b[(size_t)n * K + k];
-        const double e = std::fabs(ref - (double)d[(size_t)r * 96 + n]);
-        if (!(e <= worst)) worst = std::isnan(e) ? 1e30 : e;
-      }
-    out[ci] = worst;
-  }
   return 0;
 }
 

@@ -26,9 +26,9 @@
 //   object loop  ffn/inference/inference.py:460-533
 //   canvas loop  ffn/inference/inference.py:538-683; ffn/inference/storage.py:137-143
 //   batching     ffn/inference/executor.py:266-340 (one session.run over a [B, ...] feed)
-// Included TWICE by engine.cu: namespace FFN_KNS = plain (FFN_PROFILE 0, the product kernel) and
-// = profiled (FFN_PROFILE 1: device cycle counters, ffn_engine_profile), so that the timing code costs
-// the product kernel nothing.
+// Compiled twice, once per translation unit: flood_plain.cu defines namespace FFN_KNS = plain (FFN_PROFILE 0, the
+// product kernel) and flood_profiled.cu = profiled (FFN_PROFILE 1: device cycle counters, ffn_engine_profile), so
+// that the timing code costs the product kernel nothing.
 
 #include <math_constants.h>
 
@@ -2527,52 +2527,5 @@ __global__ void __launch_bounds__(kThreads, 1) ffn_flood_kernel(const __grid_con
 }
 
 }  // namespace FFN_KNS
-
-#ifndef FFN_MISC_KERNELS_DEFINED
-#define FFN_MISC_KERNELS_DEFINED
-// Adds `offset` to every label > 0 (multi-GPU merge, SURVEY.md 8e). HBM-bound, grid-stride.
-__global__ void relabel_offset_kernel(int* seg, size_t n, int offset) {
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const int v = seg[i];
-    if (v > 0) seg[i] = v + offset;
-  }
-}
-
-// u8 -> normalised float32 (runner.py:383-385), for ffn_canvas_read(FFN_ARRAY_IMAGE).
-__global__ void normalize_u8_kernel(const uint8_t* src, float* dst, size_t n, float mean, float stddev) {
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
-    dst[i] = __fdiv_rn(__fsub_rn((float)src[i], mean), stddev);
-}
-
-__global__ void fill_f32_kernel(float* dst, size_t n, float v) {
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) dst[i] = v;
-}
-
-// NaN-fill of a box (lo, size) of a float canvas: Canvas.init_seed's clear restricted to the touched box.
-__global__ void fill_box_f32_kernel(float* dst, int sy, int sx, int lz, int ly, int lx, int nz, int ny, int nx, float v) {
-  const size_t n = (size_t)nz * ny * nx;
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const int x = (int)(i % nx), y = (int)((i / nx) % ny), z = (int)(i / ((size_t)nx * ny));
-    dst[((size_t)(lz + z) * sy + (ly + y)) * sx + (lx + x)] = v;
-  }
-}
-
-// dst box <- src box (same canvas geometry): moves the last object's seed values into the canvas's own array.
-__global__ void copy_box_f32_kernel(float* dst, const float* src, int sy, int sx, int lz, int ly, int lx, int nz, int ny,
-                                    int nx) {
-  const size_t n = (size_t)nz * ny * nx;
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const int x = (int)(i % nx), y = (int)((i / nx) % ny), z = (int)(i / ((size_t)nx * ny));
-    const size_t a = ((size_t)(lz + z) * sy + (ly + y)) * sx + (lx + x);
-    dst[a] = src[a];
-  }
-}
-
-#endif  // FFN_MISC_KERNELS_DEFINED
 
 }  // namespace ffn

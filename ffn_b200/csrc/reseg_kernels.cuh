@@ -10,6 +10,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../../include/ffn_b200.h"
+
 namespace ffn {
 namespace rsk {
 

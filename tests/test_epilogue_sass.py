@@ -11,14 +11,11 @@ a common join.  Before the row-flag table and the per-tile addresses, every body
 F2I.TRUNC; now the three conv-layer kinds have 173-230 (the first body also holds the dispatch) and EPI_LAST, which
 also runs conv_lom and the step counts, 289-291.  The bounds leave some headroom above those counts."""
 
-import os
 import re
-import shutil
-import subprocess
 
 import pytest
 
-from ffn_b200 import build
+import flood_cubins
 
 pytestmark = pytest.mark.slow
 
@@ -27,12 +24,6 @@ kMaxLastBodyInstructions = 320   # EPI_LAST: the body with the four-lane conv_lo
 
 _INS = re.compile(r'/\*([0-9a-f]{4,})\*/\s+(.*?)\s*;')
 _BRA = re.compile(r'^(@!?U?P\w+\s+)?BRA(?:\.\w+)*\s+(0x[0-9a-f]+)$')
-
-
-def _tool(name):
-  nvcc = build.nvcc_path()
-  cand = os.path.join(os.path.dirname(nvcc), name) if os.path.isabs(nvcc) else shutil.which(name)
-  return cand if cand and os.path.exists(cand) else None
 
 
 def instructions(sass_lines):
@@ -85,15 +76,8 @@ def epilogue_bodies(ins):
 
 
 @pytest.fixture(scope='module')
-def plain_fp16_epilogues(tmp_path_factory):
-  nvcc, cuobjdump = _tool('nvcc'), _tool('cuobjdump')
-  if nvcc is None or cuobjdump is None:
-    pytest.skip('nvcc / cuobjdump not found')
-  cubin = str(tmp_path_factory.mktemp('epilogue') / 'engine.cubin')
-  res = subprocess.run([nvcc, '-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-std=c++17', '--default-stream',
-                        'per-thread', '-cubin', '-o', cubin, build.SRC], capture_output=True, text=True)
-  assert res.returncode == 0, res.stderr[-4000:]
-  sass = subprocess.run([cuobjdump, '-sass', cubin], capture_output=True, text=True, check=True).stdout
+def plain_fp16_epilogues():
+  _, sass = flood_cubins.flood_kernels()
   # ffn_flood_kernel<false> of the product namespace (<true> is the split-fp16 parity instance)
   funcs = [f for f in re.split(r'\n\s*Function : ', sass) if f.startswith('_ZN3ffn5plain16ffn_flood_kernelILb0E')]
   assert len(funcs) == 1

@@ -192,6 +192,49 @@ def test_no_cpu_fallback_without_gpu():
     eng.Engine(w, b)
 
 
+def test_standalone_entry_points_report_no_device_without_gpu():
+  # Each entry point fails in its own translation unit; the message must reach ffn_last_error in engine.cu.
+  import ctypes as C
+  import torch
+  if torch.cuda.is_available():
+    pytest.skip('GPU present')
+  lib = _lib.load()
+  p = _lib.ptr
+  n = C.c_int64(0)
+  labels = np.arange(1, 9, dtype=np.uint64)
+  dp = _lib.DecisionPointDesc(shape_zyx=(2, 2, 2), voxel_size_xyz=(1, 1, 1), box_size_zyx=(2, 2, 2))
+  rs = _lib.ResegEvalDesc(box_zyx=(2, 2, 2), voxel_size_zyx=(1, 1, 1), pair=1, num_items=1)
+  stats = np.zeros(1, _lib.RESEG_STATS_DTYPE)
+  probs, ids, table = np.zeros(16, np.uint8), np.array([1, 2], np.uint64), np.zeros(256, np.uint8)
+  pt = _lib.PartitionDesc(shape_zyx=(3, 3, 3), lom_radius_zyx=(1, 1, 1))
+  part_labels, part_out, counts = np.ones(27, np.uint64), np.zeros(1, np.uint8), np.zeros(256, np.int64)
+  pr = _lib.PartitionRowsDesc(shape_zyx=(2, 2, 2), crop_shape_zyx=(2, 2, 2))
+  volume, rows = np.zeros(8, np.uint8), np.zeros(16, np.int64)
+  names = C.create_string_buffer(b'v', 1)
+  vol = _lib.CoordinateVolume(crop_shape_zyx=(2, 2, 2), name_length=1)
+  cd = _lib.CoordinateDesc(volumes=C.cast(C.pointer(vol), C.c_void_p), n_volumes=1,
+                           names=C.cast(names, C.c_void_p), names_bytes=1)
+  records = np.zeros(64, np.uint8)
+  cu = _lib.CleanUpDesc(shape_zyx=(2, 2, 2), connectivity=1)
+  selftest = (C.c_double * 8)()
+  calls = {
+      'decision_points': lambda: lib.ffn_decision_points(0, C.byref(dp), p(labels), None, 0, C.byref(n)),
+      'reseg_eval': lambda: lib.ffn_reseg_eval(0, C.byref(rs), p(labels), p(probs), p(ids), p(table), p(stats), None, 0,
+                                               C.byref(n)),
+      'split_intersection': lambda: lib.ffn_split_intersection(0, 8, p(labels.copy()), p(labels), 0),
+      'compute_partitions': lambda: lib.ffn_compute_partitions(0, C.byref(pt), p(part_labels), None, p(part_out),
+                                                               p(counts)),
+      'partition_rows': lambda: lib.ffn_partition_rows(0, C.byref(pr), p(volume), p(rows), p(counts)),
+      'coordinate_records': lambda: lib.ffn_coordinate_records(0, C.byref(cd), p(rows), 1, p(records), records.size,
+                                                               C.byref(n)),
+      'clean_up': lambda: lib.ffn_clean_up(0, C.byref(cu), p(labels.copy()), None, None, None, 0, C.byref(n)),
+      'selftest_wgmma': lambda: lib.ffn_selftest_wgmma(0, selftest, 8),
+  }
+  for call in calls.values():
+    with pytest.raises(RuntimeError, match='no CUDA device'):
+      _lib.check(call())
+
+
 def test_canvas_rejects_foreign_executor_clients():
   from ffn.inference import executor, inference
   from ffn.training import model as ffn_model

@@ -4,22 +4,13 @@ ptxas decides for a whole function whether its wgmma instructions may stay in fl
 cannot prove that, it waits for every MMA before issuing the next one (and says so on -v).  The fp16
 kernel issues 18 MMAs per consumer warpgroup and tile, which must reach the tensor core back to back."""
 
-import os
 import re
-import shutil
-import subprocess
 
 import pytest
 
-from ffn_b200 import build
+import flood_cubins
 
 pytestmark = pytest.mark.slow
-
-
-def _tool(name):
-  nvcc = build.nvcc_path()
-  cand = os.path.join(os.path.dirname(nvcc), name) if os.path.isabs(nvcc) else shutil.which(name)
-  return cand if cand and os.path.exists(cand) else None
 
 
 def _is_fp16_flood_kernel(mangled):
@@ -28,16 +19,8 @@ def _is_fp16_flood_kernel(mangled):
 
 
 @pytest.fixture(scope='module')
-def compiled(tmp_path_factory):
-  nvcc, cuobjdump = _tool('nvcc'), _tool('cuobjdump')
-  if nvcc is None or cuobjdump is None:
-    pytest.skip('nvcc / cuobjdump not found')
-  cubin = str(tmp_path_factory.mktemp('wgmma') / 'engine.cubin')
-  res = subprocess.run([nvcc, '-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-std=c++17', '--default-stream',
-                        'per-thread', '-Xptxas', '-v', '-cubin', '-o', cubin, build.SRC], capture_output=True, text=True)
-  assert res.returncode == 0, res.stderr[-4000:]
-  sass = subprocess.run([cuobjdump, '-sass', cubin], capture_output=True, text=True, check=True).stdout
-  return res.stdout + res.stderr, sass
+def compiled():
+  return flood_cubins.flood_kernels()
 
 
 def test_fp16_flood_kernels_not_serialized(compiled):
