@@ -26,6 +26,7 @@ ARRAY_IMAGE = 3
 MASK_MOVEMENT = 0
 MASK_SEED = 1
 SEED_POLICY_KINDS = {'peaks_2d': 0, 'fill_empty': 1, 'max_peaks': 2}   # FFN_SEED_*
+OPTIMIZERS = {'sgd': 0, 'momentum': 1, 'adam': 2}   # FFN_OPT_*
 
 EXPORTS = [
     'ffn_last_error', 'ffn_engine_create', 'ffn_engine_destroy', 'ffn_engine_set_compute_mode', 'ffn_engine_set_chains', 'ffn_engine_set_grid',
@@ -35,7 +36,8 @@ EXPORTS = [
     'ffn_canvas_policy_state_size', 'ffn_canvas_policy_state_get', 'ffn_canvas_policy_state_set',
     'ffn_canvas_set_resume', 'ffn_canvas_trace', 'ffn_canvas_seed_peaks', 'ffn_canvas_seed_policy', 'ffn_canvas_set_max_id', 'ffn_canvas_get_counters', 'ffn_canvas_spec_stats', 'ffn_canvas_sched_stats', 'ffn_canvas_device_ptr',
     'ffn_canvas_add_id_offset', 'ffn_decision_points', 'ffn_reseg_eval', 'ffn_split_intersection', 'ffn_compute_partitions',
-    'ffn_partition_rows', 'ffn_coordinate_records', 'ffn_clean_up', 'ffn_selftest_wgmma',
+    'ffn_partition_rows', 'ffn_coordinate_records', 'ffn_clean_up', 'ffn_trainer_create', 'ffn_trainer_destroy',
+    'ffn_trainer_step', 'ffn_trainer_gradients', 'ffn_trainer_get_weights', 'ffn_selftest_wgmma',
 ]
 
 
@@ -93,6 +95,11 @@ class PartitionDesc(C.Structure):
 class PartitionRowsDesc(C.Structure):
   _fields_ = [('shape_zyx', C.c_int32 * 3), ('crop_start_zyx', C.c_int32 * 3), ('crop_shape_zyx', C.c_int32 * 3),
               ('reserved', C.c_int32), ('volume_index', C.c_int64)]
+
+
+class TrainDesc(C.Structure):
+  _fields_ = [('optimizer', C.c_int32), ('momentum', C.c_float), ('beta1', C.c_float), ('beta2', C.c_float),
+              ('epsilon', C.c_float), ('max_gradient_entry_mag', C.c_float), ('max_batch', C.c_int32)]
 
 
 class CleanUpDesc(C.Structure):
@@ -204,9 +211,17 @@ def load() -> C.CDLL:
   lib.ffn_coordinate_records.argtypes = [C.c_int, C.POINTER(CoordinateDesc), p, C.c_int64, p, C.c_int64,
                                          C.POINTER(C.c_int64)]
   lib.ffn_clean_up.argtypes = [C.c_int, C.POINTER(CleanUpDesc), p, p, p, p, C.c_int64, C.POINTER(C.c_int64)]
+  lib.ffn_trainer_create.argtypes = [C.c_int, C.POINTER(ModelDesc), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                     C.POINTER(TrainDesc), C.POINTER(p)]
+  lib.ffn_trainer_destroy.argtypes = [p]
+  lib.ffn_trainer_destroy.restype = None
+  lib.ffn_trainer_step.argtypes = [p, p, p, p, p, C.c_int, C.c_float, p, C.POINTER(C.c_double)]
+  lib.ffn_trainer_gradients.argtypes = [p, p, p, p, p, C.c_int, p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                        C.POINTER(C.c_double)]
+  lib.ffn_trainer_get_weights.argtypes = [p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]
   lib.ffn_selftest_wgmma.argtypes = [C.c_int, C.POINTER(C.c_double), C.c_int]
   for name in EXPORTS:
-    if name not in ('ffn_last_error', 'ffn_engine_destroy', 'ffn_canvas_destroy'):
+    if name not in ('ffn_last_error', 'ffn_engine_destroy', 'ffn_canvas_destroy', 'ffn_trainer_destroy'):
       getattr(lib, name).restype = C.c_int
   _lib = lib
   return lib

@@ -397,13 +397,7 @@ const char* ffn_last_error(void) { return g_error.c_str(); }
 int ffn_engine_create(int device, const FfnModelDesc* model, const float* const* weights_dhwio,
                       const float* const* biases, int compute_mode, FfnEngine** out) {
   if (!model || !weights_dhwio || !biases || !out) return fail("null argument");
-  if (model->features != kFeat) return fail("only 32 feature maps are supported");
-  if (model->depth < 1 || 2 * model->depth > kMaxConv) return fail("unsupported depth");
-  for (int k = 0; k < 3; ++k) {
-    if (model->fov_zyx[k] < 3 || model->fov_zyx[k] % 2 == 0) return fail("fov sizes must be odd and >= 3");
-    if (model->deltas_zyx[k] < 0 || model->deltas_zyx[k] > model->fov_zyx[k] / 2)
-      return fail("deltas must lie in [0, fov // 2]");
-  }
+  if (check_model(model)) return 1;
   cudaDeviceProp prop{};
   if (use_device(device, &prop)) return 1;
   std::unique_ptr<FfnEngine> e(new FfnEngine());

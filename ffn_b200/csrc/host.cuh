@@ -1,5 +1,5 @@
 // host.cuh — the host-side idiom of every entry point: errors (fail, CUDA_OK), device selection (use_device), device
-// memory (DevBufs) and CUB scratch (CubTemp).
+// memory (DevBufs), CUB scratch (CubTemp) and the checks of a model description (check_model).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -7,6 +7,8 @@
 #include <algorithm>
 #include <string>
 #include <vector>
+
+#include "device_types.cuh"
 
 namespace ffn {
 
@@ -88,6 +90,18 @@ inline int use_device(int device, cudaDeviceProp* prop) {
     return fail(std::string("device is sm_") + std::to_string(prop->major) + std::to_string(prop->minor) +
                 "; this library only contains sm_90a code");
   CUDA_OK(cudaSetDevice(device));
+  return 0;
+}
+
+// The ConvStack3DFFNModel geometries the library runs, for engines and trainers alike.
+inline int check_model(const FfnModelDesc* model) {
+  if (model->features != kFeat) return fail("only 32 feature maps are supported");
+  if (model->depth < 1 || 2 * model->depth > kMaxConv) return fail("unsupported depth");
+  for (int k = 0; k < 3; ++k) {
+    if (model->fov_zyx[k] < 3 || model->fov_zyx[k] % 2 == 0) return fail("fov sizes must be odd and >= 3");
+    if (model->deltas_zyx[k] < 0 || model->deltas_zyx[k] > model->fov_zyx[k] / 2)
+      return fail("deltas must lie in [0, fov // 2]");
+  }
   return 0;
 }
 

@@ -445,6 +445,41 @@ typedef struct {
 int ffn_clean_up(int device, const FfnCleanUpDesc* desc, uint64_t* labels, uint64_t* ids, uint64_t* orig_ids,
                  int64_t* counts, int64_t cap, int64_t* n_ids);
 
+/* ---- training step: train.py:135-152 with model.py:115-157 and optimizer.py:73-112 ---------------------------------
+ * One sess.run([train_op, global_step, logits]) of the reference's train.py on a batch of field-of-view patches:
+ * forward pass, mean(sigmoid_cross_entropy_with_logits(logits, labels) * loss_weights) over all batch * Z * Y * X
+ * elements, backward pass, every gradient entry clipped to +-max_gradient_entry_mag, one optimizer step.  The 3x3x3
+ * convolutions run on the tensor cores with bf16 operands and fp32 accumulation; the residual stream, conv_lom, the
+ * weights, biases and optimizer slots are fp32.  Every reduction runs in a fixed order: two identical steps give
+ * bit-identical weights. */
+typedef struct FfnTrainer FfnTrainer;
+enum { FFN_OPT_SGD = 0, FFN_OPT_MOMENTUM = 1, FFN_OPT_ADAM = 2 };
+typedef struct {
+  int32_t optimizer;              /* FFN_OPT_* */
+  float momentum;                 /* momentum: MomentumOptimizer's momentum (not Nesterov) */
+  float beta1, beta2, epsilon;    /* adam: AdamOptimizer's beta1, beta2, epsilon */
+  float max_gradient_entry_mag;   /* <= 0: no clipping */
+  int32_t max_batch;              /* patches per call the trainer allocates for */
+} FfnTrainDesc;
+/* weights_dhwio / biases as for ffn_engine_create; the model checks are those of ffn_engine_create.  The trainer keeps
+ * its own fp32 copy of the weights and the optimizer slots (zero), and owns all its device memory. */
+int ffn_trainer_create(int device, const FfnModelDesc* model, const float* const* weights_dhwio,
+                       const float* const* biases, const FfnTrainDesc* desc, FfnTrainer** out);
+void ffn_trainer_destroy(FfnTrainer* trainer);
+/* seed, image, labels, loss_weights (NULL: all 1): host float32 [batch, Z, Y, X], 1 <= batch <= max_batch.  Runs the
+ * step at learning_rate (the host applies any decay) and advances the global step.  logits_out (NULL: not returned):
+ * the logits of the weights before the update.  *loss_out: the loss, summed in float64. */
+int ffn_trainer_step(FfnTrainer* trainer, const float* seed, const float* image, const float* labels,
+                     const float* loss_weights, int batch, float learning_rate, float* logits_out, double* loss_out);
+/* The same forward and backward pass without the update: d loss / d logits [batch, Z, Y, X] and the raw (unclipped)
+ * gradients in the layout of weights_dhwio / biases (any pointer may be NULL).  Changes nothing. */
+int ffn_trainer_gradients(FfnTrainer* trainer, const float* seed, const float* image, const float* labels,
+                          const float* loss_weights, int batch, float* dlogits_out, float* const* weight_grads,
+                          float* const* bias_grads, double* loss_out);
+/* The current weights in the layout ffn_engine_create takes, and the number of steps run. */
+int ffn_trainer_get_weights(FfnTrainer* trainer, float* const* weights_dhwio, float* const* biases,
+                            int64_t* global_step);
+
 /* Known-answer test of the wgmma descriptors (worst absolute error of each case in out[]; see
  * ffn_selftest_wgmma in ffn_b200/csrc/engine.cu).  Used by tests, not by the product path. */
 int ffn_selftest_wgmma(int device, double* out, int n_out);
