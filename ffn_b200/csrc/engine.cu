@@ -422,10 +422,16 @@ int ffn_engine_create(int device, const FfnModelDesc* model, const float* const*
   e->smem_bytes = L.total;
   if ((size_t)L.total > prop.sharedMemPerBlockOptin)
     return fail("field of view too large for the shared-memory operand staging");
+  // The dynamic shared-memory cap belongs to the kernel, not to this engine: it is set to all a block may use, so that
+  // creating an engine of a smaller field of view never lowers it below a larger engine's launches.  Occupancy is
+  // checked at this engine's own size.
   for (const bool profiling : {false, true})
     for (const bool split : {false, true}) {
       const void* k = flood_kernel(profiling, split);
-      CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total));
+      cudaFuncAttributes attr{};
+      CUDA_OK(cudaFuncGetAttributes(&attr, k));
+      CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)(prop.sharedMemPerBlockOptin - attr.sharedSizeBytes)));
       int per_sm = 0;
       CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, kThreads, L.total));
       if (per_sm < 1) return fail("persistent kernel does not fit on an SM");

@@ -209,10 +209,12 @@ int ffn_trainer_create(int device, const FfnModelDesc* model, const float* const
                                                {(const void*)trk::conv<4, trk::kFwdB>, 4},
                                                {(const void*)trk::conv<4, trk::kBwdA>, 4},
                                                {(const void*)trk::conv<4, trk::kBwdB>, 4}};
-  for (const auto& k : convs) {
+  size_t conv_static[5];
+  for (int i = 0; i < 5; ++i) {
     cudaFuncAttributes attr{};
-    CUDA_OK(cudaFuncGetAttributes(&attr, k.first));
-    if (conv_smem(g, k.second) + attr.sharedSizeBytes > prop.sharedMemPerBlockOptin)
+    CUDA_OK(cudaFuncGetAttributes(&attr, convs[i].first));
+    conv_static[i] = attr.sharedSizeBytes;
+    if (conv_smem(g, convs[i].second) + attr.sharedSizeBytes > prop.sharedMemPerBlockOptin)
       return fail("field of view too wide for the conv kernel's staging");
   }
 
@@ -265,8 +267,11 @@ int ffn_trainer_create(int device, const FfnModelDesc* model, const float* const
       m.get(&t->bpart, (size_t)gmax.data_rows / trk::kTileRows * 32) || m.get(&t->hpart, (size_t)hb * trk::kHeadCols) ||
       m.get(&t->hsum, trk::kHeadCols) || m.get(&t->lpart, hb))
     return 1;
-  for (const auto& k : convs)
-    CUDA_OK(cudaFuncSetAttribute(k.first, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)conv_smem(g, k.second)));
+  // The dynamic shared-memory cap belongs to the kernel, not to this trainer: it is set to all a block may use, so that
+  // creating a trainer of a narrower field of view never lowers it below a wider trainer's launches.
+  for (int i = 0; i < 5; ++i)
+    CUDA_OK(cudaFuncSetAttribute(convs[i].first, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)(prop.sharedMemPerBlockOptin - conv_static[i])));
   CUDA_OK(cudaFuncSetAttribute(trk::wgrad<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, trk::WgradShape<2>::kSmem));
   CUDA_OK(cudaFuncSetAttribute(trk::wgrad<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, trk::WgradShape<4>::kSmem));
   CUDA_OK(cudaDeviceSynchronize());

@@ -97,3 +97,31 @@ def test_device_memory_returns_to_the_first_cycle_level(cycles):
     pytest.skip('NVML lists no compute process with pid %d (in a container NVML may report the process under another '
                 'pid), or NVML is unavailable: memory not checked' % os.getpid())
   assert memory[-1] <= memory[0], memory
+
+
+def test_a_smaller_engine_leaves_a_larger_ones_launches_alone(golden_dir):
+  """An engine of a smaller field of view created after a larger one must not lower what the larger one's flood-kernel
+  launches may use: the larger engine's predict and segment_at give what they gave before the smaller one existed."""
+  from ffn_b200 import _lib, engine as eng, tf_checkpoint
+  w, b = tf_checkpoint.load_convstack_npz(os.path.join(golden_dir, 'fib25_convstack.npz'))
+  vol = np.load(os.path.join(golden_dir, 'flood_fill_64.npz'))['volume']
+  rng = np.random.RandomState(1)
+  seed, image = rng.uniform(0.0, 1.0, (2,) + FOV).astype(np.float32), rng.randn(2, *FOV).astype(np.float32)
+  large = eng.Engine(w, b, FOV, DELTAS, compute_mode=_lib.COMPUTE_FP16_TC)
+
+  def run():
+    logits = large.predict(seed, image)
+    cv = eng.DeviceCanvas(large, vol, eng.make_options(), 128.0, 33.0)
+    steps = cv.segment_at((16, 48, 32), max_steps=6).iters
+    out = cv.read(_lib.ARRAY_SEED)
+    cv.close()
+    return logits, steps, out
+
+  before = run()
+  small = eng.Engine(w, b, (3, 3, 3), (1, 1, 1), compute_mode=_lib.COMPUTE_FP16_TC)
+  after = run()
+  small.close()
+  large.close()
+  assert after[1] == before[1] == 6
+  np.testing.assert_array_equal(after[0], before[0])
+  np.testing.assert_array_equal(after[2], before[2])

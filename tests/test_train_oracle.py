@@ -9,6 +9,7 @@ import tempfile
 import numpy as np
 import pytest
 import torch
+import torch.nn.functional as F
 
 import train_cases
 from oracle import exact_net, network, train_step as ts
@@ -16,24 +17,10 @@ from oracle import exact_net, network, train_step as ts
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _net(depth, seed, scale=0.2):
-  rng = np.random.RandomState(seed)
-  w = [(rng.randn(3, 3, 3, 2 if i == 0 else 32, 32) * scale).astype(np.float32) for i in range(2 * depth)]
-  w.append((rng.randn(1, 1, 1, 32, 1) * scale).astype(np.float32))
-  b = [(rng.randn(32) * 0.1).astype(np.float32) for _ in range(2 * depth)] + [np.float32([0.1])]
-  return w, b
-
-
-def _batch(fov, n, seed):
-  rng = np.random.RandomState(seed)
-  return tuple(a.astype(np.float32) for a in (rng.randn(n, *fov), rng.randn(n, *fov), rng.uniform(0, 1, (n,) + fov),
-                                              rng.uniform(0.5, 2, (n,) + fov)))
-
-
 @pytest.mark.parametrize('depth', [1, 2])
 def test_gradients_equal_central_differences(depth):
-  w, b = _net(depth, depth)
-  seed, image, labels, lw = _batch((5, 5, 5), 2, 3)
+  w, b = train_cases.real_net(depth, depth)
+  seed, image, labels, lw = train_cases.real_batch((5, 5, 5), 2, 3)
   _, _, gw, gb, loss = ts.gradients(w, b, seed, image, labels, lw)
   rng = np.random.RandomState(4)
   h = 1e-6
@@ -51,8 +38,8 @@ def test_gradients_equal_central_differences(depth):
 
 
 def test_forward_logits_equal_the_network_oracle():
-  w, b = _net(3, 7)
-  seed, image, _, _ = _batch((7, 9, 5), 2, 8)
+  w, b = train_cases.real_net(3, 7)
+  seed, image, _, _ = train_cases.real_batch((7, 9, 5), 2, 8)
   got = ts.gradients(w, b, seed, image, dlogits=np.zeros(seed.shape))[0]
   want = network.ConvStackOracle(w, b, dtype=torch.float64).update(seed, image) + seed
   np.testing.assert_allclose(got, want, rtol=1e-12, atol=1e-12)
@@ -81,6 +68,10 @@ def test_optimizer_formulas_by_hand():
 def test_bf16_rounding_is_round_to_nearest_even():
   x = np.array([1 + 2 ** -8, 1 + 3 * 2 ** -8, 1 + 2 ** -8 + 2 ** -20, -(1 + 2 ** -8), 2 ** -130])
   np.testing.assert_array_equal(ts.round_bf16(x), [1, 1 + 2 ** -6, 1 + 2 ** -7, -1, 2 ** -130])
+  # the wrong modes of the bugs 'bf16_truncate' and 'bf16_half_away'
+  np.testing.assert_array_equal(ts.round_bf16(x, 'rtz'), [1, 1 + 2 ** -7, 1, -1, 2 ** -130])
+  np.testing.assert_array_equal(ts.round_bf16(x, 'rha'), [1 + 2 ** -7, 1 + 2 ** -6, 1 + 2 ** -7, -(1 + 2 ** -7),
+                                                          2 ** -130])
 
 
 def test_exact_case_satisfies_the_premise_and_large_sums_are_rejected():
@@ -92,27 +83,50 @@ def test_exact_case_satisfies_the_premise_and_large_sums_are_rejected():
   assert 'conv2 forward' in names and any('wgrad' in n for n in names)
 
 
-def _zero_preactivation_case():
-  """An exact step in which conv0_a's channel 0 is exactly 0 at every voxel: a constant image of 1/2 and bias -1/2."""
-  w, b, seed, image, labels, lw, dl = train_cases.exact_case((3, 5, 5), 2, 1, density=1.0)
-  w[0][...] = 0
-  w[0][1, 1, 1, 0, 0] = 1.0
-  w[1][:, :, :, 0, :] = 1.0
-  b[0][0] = -0.5
-  return w, b, seed, np.full_like(image, 0.5), dl
+@pytest.mark.parametrize('name', sorted(train_cases.PROBE_BUGS))
+def test_every_probe_satisfies_the_premise(name):
+  w, b, seed, image, labels, lw, dl = train_cases.probe(name)
+  assert not ts.premise_violations(w, b, seed, image, dl)
+  assert np.count_nonzero(dl) > dl.size // 3
 
 
 @pytest.mark.parametrize('bug', ts.BUGS)
 def test_each_probe_bug_changes_a_gradient(bug):
-  """The bugs the exact GPU test catches though a tolerance would not: a ReLU derivative of 1 at a pre-activation of
-  exactly 0, a residual gradient not carried past the skip, and an input gradient without the tap flip."""
-  if bug == 'relu_grad_at_zero':
-    w, b, seed, image, dl = _zero_preactivation_case()
-  else:
-    w, b, seed, image, _, _, dl = train_cases.exact_case((5, 5, 7), 2, 1, density=1.0)
-  _, _, rw, rb, _ = ts.gradients(w, b, seed, image, dlogits=dl, bf16=True)
-  _, _, bw, bb, _ = ts.gradients(w, b, seed, image, dlogits=dl, bf16=True, bug=bug)
-  assert any(not np.array_equal(x, y) for x, y in zip(rw + rb, bw + bb))
+  """The bugs the exact GPU tests catch though a tolerance would not, each on every probe listed for it: a ReLU
+  derivative of 1 at a pre-activation of exactly 0, a residual gradient not carried past the skip, an input gradient
+  without the tap flip, a wrong bf16 rounding mode, bias gradients of the rounded output gradient, a residual gradient
+  rounded to bf16 and a rounded seed in the head.  Each changes the logits or a gradient."""
+  names = [n for n, bugs in train_cases.PROBE_BUGS.items() if bug in bugs]
+  assert names
+  for name in names:
+    w, b, seed, image, _, _, dl = train_cases.probe(name)
+    rl, _, rw, rb, _ = ts.gradients(w, b, seed, image, dlogits=dl, bf16=True)
+    bl, _, bw, bb, _ = ts.gradients(w, b, seed, image, dlogits=dl, bf16=True, bug=bug)
+    assert any(not np.array_equal(x, y) for x, y in zip([rl] + rw + rb, [bl] + bw + bb)), name
+
+
+def test_loss_gradient_at_logit_zero_is_one_half_minus_the_label():
+  """At x = 0 the derivative is sigmoid(0) - z = 1/2 - z (autograd of TF's formula would take 1 - z there)."""
+  w, b, seed, image, labels, lw, dl = train_cases.exact_case((3, 5, 7), 1, 2, density=0.5)
+  logits, got, _, _, _ = ts.gradients(w, b, seed, image, labels, lw, bf16=True)
+  np.testing.assert_array_equal(logits, 0)
+  np.testing.assert_array_equal(got, dl)
+
+
+def test_head_reference_equals_sigmoid_xent_and_autograd():
+  w, b, seed, image, labels, lw = train_cases.head_grid_case()
+  ref = ts.head_reference(seed, labels, lw)
+  x = torch.from_numpy(seed.astype(np.float64)).requires_grad_()
+  loss = ts.sigmoid_xent(x, labels, lw)
+  loss.backward()
+  assert abs(float(loss.detach()) - ref['loss']) <= 1e-12 * abs(ref['loss'])
+  np.testing.assert_allclose(x.grad.numpy(), ref['dlogits'], rtol=1e-12, atol=0)
+  # conv_lom's sums against the oracle's backward pass of the same step (w_lom = b_lom = 0: logits = seed)
+  act = F.relu(ts.forward(*ts._params(w, b), seed, image, bf16=True)[1]).detach().numpy()
+  ref = ts.head_reference(seed, labels, lw, act)
+  _, _, gw, gb, _ = ts.gradients(w, b, seed, image, labels, lw, bf16=True)
+  np.testing.assert_allclose(gw[-1].reshape(-1), ref['w_lom'], rtol=1e-12, atol=0)
+  assert abs(gb[-1][0] - ref['b_lom']) <= 1e-12 * np.abs(ref['dlogits']).sum()
 
 
 @pytest.mark.slow
