@@ -37,7 +37,8 @@ EXPORTS = [
     'ffn_canvas_set_resume', 'ffn_canvas_trace', 'ffn_canvas_seed_peaks', 'ffn_canvas_seed_policy', 'ffn_canvas_set_max_id', 'ffn_canvas_get_counters', 'ffn_canvas_spec_stats', 'ffn_canvas_sched_stats', 'ffn_canvas_device_ptr',
     'ffn_canvas_add_id_offset', 'ffn_decision_points', 'ffn_reseg_eval', 'ffn_split_intersection', 'ffn_compute_partitions',
     'ffn_partition_rows', 'ffn_coordinate_records', 'ffn_clean_up', 'ffn_trainer_create', 'ffn_trainer_destroy',
-    'ffn_trainer_step', 'ffn_trainer_gradients', 'ffn_trainer_get_weights', 'ffn_selftest_wgmma',
+    'ffn_trainer_step', 'ffn_trainer_gradients', 'ffn_trainer_get_weights', 'ffn_trainer_train', 'ffn_examples_create',
+    'ffn_examples_destroy', 'ffn_examples_next', 'ffn_examples_update', 'ffn_examples_read_seeds', 'ffn_selftest_wgmma',
 ]
 
 
@@ -100,6 +101,24 @@ class PartitionRowsDesc(C.Structure):
 class TrainDesc(C.Structure):
   _fields_ = [('optimizer', C.c_int32), ('momentum', C.c_float), ('beta1', C.c_float), ('beta2', C.c_float),
               ('epsilon', C.c_float), ('max_gradient_entry_mag', C.c_float), ('max_batch', C.c_int32)]
+
+
+FOV_POLICIES = {'fixed': 0, 'max_pred_moves': 1}   # FFN_FOV_*
+# FfnExampleCoord, as a numpy record so that a stream of them is one contiguous array
+EXAMPLE_COORD_DTYPE = np.dtype([('volume', '<i4'), ('center_xyz', '<i4', (3,)), ('permutation_zyx', '<i4', (3,)),
+                                ('reflect_zyx', '<i4', (3,))])
+
+
+class ExampleVolume(C.Structure):
+  _fields_ = [('image', C.c_void_p), ('labels', C.c_void_p), ('image_shape_zyx', C.c_int32 * 3),
+              ('label_shape_zyx', C.c_int32 * 3), ('offset', C.c_float), ('scale', C.c_float)]
+
+
+class ExampleDesc(C.Structure):
+  _fields_ = [('policy', C.c_int32), ('fov_moves', C.c_int32), ('seed_pad', C.c_float), ('seed_logit_pad', C.c_float),
+              ('seed_logit_centre', C.c_float), ('batch', C.c_int32), ('seed_threshold', C.c_double),
+              ('label_threshold', C.c_double), ('shifts_zyx', C.c_void_p), ('n_shifts', C.c_int32),
+              ('permutable_zyx', C.c_int32 * 3), ('reflectable_zyx', C.c_int32 * 3)]
 
 
 class CleanUpDesc(C.Structure):
@@ -219,9 +238,17 @@ def load() -> C.CDLL:
   lib.ffn_trainer_gradients.argtypes = [p, p, p, p, p, C.c_int, p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
                                         C.POINTER(C.c_double)]
   lib.ffn_trainer_get_weights.argtypes = [p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]
+  lib.ffn_trainer_train.argtypes = [p, p, p, C.c_int64, C.c_int, p, p, C.POINTER(C.c_int64)]
+  lib.ffn_examples_create.argtypes = [C.c_int, C.POINTER(ModelDesc), C.POINTER(ExampleDesc), p, C.c_int, C.POINTER(p)]
+  lib.ffn_examples_destroy.argtypes = [p]
+  lib.ffn_examples_destroy.restype = None
+  lib.ffn_examples_next.argtypes = [p, p, C.c_int64, p, p, p, p, p, C.POINTER(C.c_int64)]
+  lib.ffn_examples_update.argtypes = [p, p]
+  lib.ffn_examples_read_seeds.argtypes = [p, p]
   lib.ffn_selftest_wgmma.argtypes = [C.c_int, C.POINTER(C.c_double), C.c_int]
   for name in EXPORTS:
-    if name not in ('ffn_last_error', 'ffn_engine_destroy', 'ffn_canvas_destroy', 'ffn_trainer_destroy'):
+    if name not in ('ffn_last_error', 'ffn_engine_destroy', 'ffn_canvas_destroy', 'ffn_trainer_destroy',
+                    'ffn_examples_destroy'):
       getattr(lib, name).restype = C.c_int
   _lib = lib
   return lib

@@ -105,4 +105,13 @@ inline int check_model(const FfnModelDesc* model) {
   return 0;
 }
 
+// The training example loop's steps that ffn_trainer_train runs (defined in examples.cu).  All work is enqueued on
+// cudaStreamPerThread; examples_finish reads the call's results after a synchronisation.
+int examples_check_trainer(const FfnExamples* ex, int device, const int fov_zyx[3], int max_batch);
+int examples_batch(const FfnExamples* ex);
+int examples_upload(FfnExamples* ex, const FfnExampleCoord* coords, int64_t n);
+int examples_advance(FfnExamples* ex, float* seed, float* image, float* labels);
+int examples_paste(FfnExamples* ex, const float* logits);
+int examples_finish(FfnExamples* ex, int64_t* n_consumed);
+
 }  // namespace ffn

@@ -72,22 +72,15 @@ int launch_wgrad(FfnTrainer* t, const TGeom& g, int l) {
   return launch_reduce(t->wpart, g.data_rows / trk::kSplitRows, 27 * cin_of(l) * 32, t->grads + t->w_off[l]);
 }
 
-// Forward, loss and backward of one batch: logits, dlogits and the raw gradients of every parameter on the device.
-int run(FfnTrainer* t, const float* seed, const float* image, const float* labels, const float* loss_weights, int batch,
-        double* loss_out) {
-  if (!seed || !image || !labels) return fail("null argument");
-  if (batch < 1 || batch > t->max_batch)
-    return fail("batch " + std::to_string(batch) + " outside [1, " + std::to_string(t->max_batch) + "]");
-  CUDA_OK(cudaSetDevice(t->device));
+// Forward, loss and backward of the batch in t->seed, t->image, t->labels (and t->lw when use_lw): logits, dlogits,
+// the raw gradients of every parameter and the head's loss partial sums (t->lpart, *hb_out of them), on the device.
+// Enqueues only; nothing is synchronised.
+int run_device(FfnTrainer* t, bool use_lw, int batch, int* hb_out) {
   cudaStream_t st = cudaStreamPerThread;
   TGeom g = t->g;
   g.batch = batch;
   g.data_rows = data_rows(g, batch);
   const size_t nv = (size_t)batch * g.V;
-  CUDA_OK(cudaMemcpyAsync(t->seed, seed, nv * 4, cudaMemcpyHostToDevice, st));
-  CUDA_OK(cudaMemcpyAsync(t->image, image, nv * 4, cudaMemcpyHostToDevice, st));
-  CUDA_OK(cudaMemcpyAsync(t->labels, labels, nv * 4, cudaMemcpyHostToDevice, st));
-  if (loss_weights) CUDA_OK(cudaMemcpyAsync(t->lw, loss_weights, nv * 4, cudaMemcpyHostToDevice, st));
   const int blocks = t->sm_count * 4;
   for (int l = 0; l < t->nconv; ++l)
     trk::pack_weights<<<blocks, 256, 0, st>>>(t->params + t->w_off[l], cin_of(l), kc_of(l), t->wf[l], t->wt[l]);
@@ -114,7 +107,7 @@ int run(FfnTrainer* t, const float* seed, const float* image, const float* label
   trk::HeadArgs h{};
   h.seed = t->seed;
   h.labels = t->labels;
-  h.loss_weights = loss_weights ? t->lw : nullptr;
+  h.loss_weights = use_lw ? t->lw : nullptr;
   h.res = t->res;
   h.mask = t->mask[t->nconv];
   h.lom = t->params + t->w_off[t->nconv];
@@ -155,6 +148,25 @@ int run(FfnTrainer* t, const float* seed, const float* image, const float* label
     if (launch_reduce(t->bpart, ntiles, 32, t->grads + t->b_off[l - 1])) return 1;
     std::swap(t->gout[0], t->gout[1]);
   }
+  *hb_out = hb;
+  return 0;
+}
+
+// run_device on a batch copied from the host, and the loss summed on the host.
+int run(FfnTrainer* t, const float* seed, const float* image, const float* labels, const float* loss_weights, int batch,
+        double* loss_out) {
+  if (!seed || !image || !labels) return fail("null argument");
+  if (batch < 1 || batch > t->max_batch)
+    return fail("batch " + std::to_string(batch) + " outside [1, " + std::to_string(t->max_batch) + "]");
+  CUDA_OK(cudaSetDevice(t->device));
+  cudaStream_t st = cudaStreamPerThread;
+  const size_t nv = (size_t)batch * t->g.V;
+  CUDA_OK(cudaMemcpyAsync(t->seed, seed, nv * 4, cudaMemcpyHostToDevice, st));
+  CUDA_OK(cudaMemcpyAsync(t->image, image, nv * 4, cudaMemcpyHostToDevice, st));
+  CUDA_OK(cudaMemcpyAsync(t->labels, labels, nv * 4, cudaMemcpyHostToDevice, st));
+  if (loss_weights) CUDA_OK(cudaMemcpyAsync(t->lw, loss_weights, nv * 4, cudaMemcpyHostToDevice, st));
+  int hb = 0;
+  if (run_device(t, loss_weights != nullptr, batch, &hb)) return 1;
   std::vector<double> lp(hb);
   CUDA_OK(cudaMemcpyAsync(lp.data(), t->lpart, hb * sizeof(double), cudaMemcpyDeviceToHost, st));
   CUDA_OK(cudaStreamSynchronize(st));
@@ -162,6 +174,40 @@ int run(FfnTrainer* t, const float* seed, const float* image, const float* label
   for (double v : lp) s += v;
   if (loss_out) *loss_out = s / (double)nv;
   return 0;
+}
+
+// Enqueues the optimizer step at learning_rate on the gradients in t->grads, and advances the global step and Adam's
+// beta powers (the host forms Adam's alpha from them, in float32).
+int launch_update(FfnTrainer* t, float learning_rate) {
+  trk::UpdateArgs u{};
+  u.w = t->params;
+  u.a = t->slot_a;
+  u.b = t->slot_b;
+  u.grad = t->grads;
+  u.n = t->nparam;
+  u.optimizer = t->desc.optimizer;
+  u.clip = t->desc.max_gradient_entry_mag;
+  u.lr = learning_rate;
+  u.momentum = t->desc.momentum;
+  u.one_minus_b1 = 1.0f - t->desc.beta1;
+  u.one_minus_b2 = 1.0f - t->desc.beta2;
+  u.alpha = learning_rate * std::sqrt(1.0f - t->beta2_power) / (1.0f - t->beta1_power);
+  u.eps = t->desc.epsilon;
+  trk::update<<<t->sm_count * 4, 256, 0, cudaStreamPerThread>>>(u);
+  CUDA_OK(cudaGetLastError());
+  t->global_step++;
+  if (t->desc.optimizer == FFN_OPT_ADAM) {
+    t->beta1_power = t->beta1_power * t->desc.beta1;
+    t->beta2_power = t->beta2_power * t->desc.beta2;
+  }
+  return 0;
+}
+
+// The loss of one step: the head's partial sums added in the order ffn_trainer_step adds them on the host.
+__global__ void sum_loss(const double* part, int n, double nv, double* out) {
+  double s = 0.0;
+  for (int i = 0; i < n; ++i) s = __dadd_rn(s, part[i]);
+  *out = __ddiv_rn(s, nv);
 }
 
 int copy_params(const FfnTrainer* t, const float* src, float* const* w, float* const* b) {
@@ -285,31 +331,11 @@ int ffn_trainer_step(FfnTrainer* t, const float* seed, const float* image, const
                      const float* loss_weights, int batch, float learning_rate, float* logits_out, double* loss_out) {
   if (!t) return fail("null trainer");
   if (run(t, seed, image, labels, loss_weights, batch, loss_out)) return 1;
-  trk::UpdateArgs u{};
-  u.w = t->params;
-  u.a = t->slot_a;
-  u.b = t->slot_b;
-  u.grad = t->grads;
-  u.n = t->nparam;
-  u.optimizer = t->desc.optimizer;
-  u.clip = t->desc.max_gradient_entry_mag;
-  u.lr = learning_rate;
-  u.momentum = t->desc.momentum;
-  u.one_minus_b1 = 1.0f - t->desc.beta1;
-  u.one_minus_b2 = 1.0f - t->desc.beta2;
-  u.alpha = learning_rate * std::sqrt(1.0f - t->beta2_power) / (1.0f - t->beta1_power);
-  u.eps = t->desc.epsilon;
-  trk::update<<<t->sm_count * 4, 256, 0, cudaStreamPerThread>>>(u);
-  CUDA_OK(cudaGetLastError());
+  if (launch_update(t, learning_rate)) return 1;
   if (logits_out)
     CUDA_OK(cudaMemcpyAsync(logits_out, t->logits, (size_t)batch * t->g.V * 4, cudaMemcpyDeviceToHost,
                             cudaStreamPerThread));
   CUDA_OK(cudaStreamSynchronize(cudaStreamPerThread));
-  t->global_step++;
-  if (t->desc.optimizer == FFN_OPT_ADAM) {
-    t->beta1_power = t->beta1_power * t->desc.beta1;
-    t->beta2_power = t->beta2_power * t->desc.beta2;
-  }
   return 0;
 }
 
@@ -321,6 +347,34 @@ int ffn_trainer_gradients(FfnTrainer* t, const float* seed, const float* image, 
   if (dlogits_out)
     CUDA_OK(cudaMemcpyAsync(dlogits_out, t->dl, (size_t)batch * t->g.V * 4, cudaMemcpyDeviceToHost, cudaStreamPerThread));
   return copy_params(t, t->grads, weight_grads, bias_grads);
+}
+
+int ffn_trainer_train(FfnTrainer* t, FfnExamples* ex, const FfnExampleCoord* coords, int64_t n_coords, int n_steps,
+                      const float* learning_rate, double* losses_out, int64_t* n_consumed) {
+  if (!t || !ex || !coords || (n_steps > 0 && (!learning_rate || !losses_out))) return fail("null argument");
+  if (n_steps < 0) return fail("negative n_steps");
+  const int fov[3] = {t->g.Z, t->g.Y, t->g.X};
+  if (examples_check_trainer(ex, t->device, fov, t->max_batch)) return 1;
+  const int batch = examples_batch(ex);
+  if (n_coords < (int64_t)n_steps * batch)
+    return fail("a step may take one stream entry per element: pass at least n_steps * batch (" +
+                std::to_string((int64_t)n_steps * batch) + ") entries");
+  CUDA_OK(cudaSetDevice(t->device));
+  cudaStream_t st = cudaStreamPerThread;
+  DevBufs tmp;
+  double* losses = nullptr;
+  if (tmp.get(&losses, n_steps) || examples_upload(ex, coords, (int64_t)n_steps * batch)) return 1;
+  const double nv = (double)((size_t)batch * t->g.V);
+  for (int i = 0; i < n_steps; ++i) {
+    int hb = 0;
+    if (examples_advance(ex, t->seed, t->image, t->labels) || run_device(t, false, batch, &hb)) return 1;
+    sum_loss<<<1, 1, 0, st>>>(t->lpart, hb, nv, losses + i);
+    CUDA_OK(cudaGetLastError());
+    if (launch_update(t, learning_rate[i]) || examples_paste(ex, t->logits)) return 1;
+  }
+  if (n_steps) CUDA_OK(cudaMemcpyAsync(losses_out, losses, n_steps * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+  return examples_finish(ex, n_consumed);
 }
 
 int ffn_trainer_get_weights(FfnTrainer* t, float* const* weights_dhwio, float* const* biases, int64_t* global_step) {

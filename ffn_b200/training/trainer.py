@@ -131,6 +131,24 @@ class Trainer:
                                                self._ptrs(gw), self._ptrs(gb), C.byref(loss)))
     return dl, gw, gb, float(loss.value)
 
+  def train(self, loop, n_steps: int) -> np.ndarray:
+    """n_steps training steps fed by an ExampleLoop, on the device with one host synchronisation: per step the loop's
+    next batch, `step` on it with unit loss weights, and the logits pasted back into the seeds.  Each step's learning
+    rate is the decayed rate at its global step.  Returns the losses, each equal to `step`'s bit for bit."""
+    n_steps = int(n_steps)
+    if n_steps < 0:
+      raise ValueError('n_steps must not be negative')
+    step0 = self.global_step
+    lr = np.array([decayed_learning_rate(self.learning_rate, step0 + i, self.learning_rate_decay_factor,
+                                         self.decay_steps) for i in range(n_steps)], np.float32)
+    coords = loop.entries(n_steps * loop.batch_size)
+    losses = np.zeros(n_steps, np.float64)
+    n = C.c_int64()
+    _lib.check(self._lib.ffn_trainer_train(self._h, loop.handle, _lib.ptr(coords), len(coords), n_steps,
+                                           _lib.ptr(lr), _lib.ptr(losses), C.byref(n)))
+    loop.consume(int(n.value))
+    return losses
+
   def weights(self):
     """(weights, biases) in the layout `Engine` and ffn_b200/tf_checkpoint.py use."""
     ws = [np.empty(sh, np.float32) for sh in self.shapes[0]]

@@ -480,6 +480,69 @@ int ffn_trainer_gradients(FfnTrainer* trainer, const float* seed, const float* i
 int ffn_trainer_get_weights(FfnTrainer* trainer, float* const* weights_dhwio, float* const* biases,
                             int64_t* global_step);
 
+/* ---- training examples: train.py:202-286, 353-412 and ffn/training/examples.py ------------------------------------
+ * The example loop of the reference's train.py, resident on the device: per batch element a training patch (image,
+ * softened labels and the seed canvas, each fov + 2 * deltas * moves voxels per axis, with moves = fov_moves for the
+ * fixed policy and fov_moves + 1 for max_pred_moves), the offset of its field of view and the state of its move policy.
+ * One step pastes the previous step's logits into the seed, resumes the policy on the updated seed and, when it is
+ * exhausted, loads the next example of the coordinate stream (crop, object mask of the centre label, 0.95 / 0.05
+ * labels, the example's axis permutation and reflections, (image - offset) / scale in float32).  New examples go to
+ * the elements in element order 0 .. batch-1 within a step.  A fresh example always yields its centre, so an element
+ * takes at most one new example per step. */
+typedef struct FfnExamples FfnExamples;
+enum { FFN_FOV_FIXED = 0, FFN_FOV_MAX_PRED_MOVES = 1 };
+typedef struct {
+  int32_t volume;                 /* index into the volumes given to ffn_examples_create */
+  int32_t center_xyz[3];          /* the crop is centre - (size - 1) // 2 .. + size */
+  int32_t permutation_zyx[3];     /* axis i of the example is axis permutation_zyx[i] of the crop (np.transpose) */
+  int32_t reflect_zyx[3];         /* nonzero: that axis is reversed after the permutation */
+} FfnExampleCoord;
+typedef struct {
+  const uint8_t* image;           /* host [z][y][x] */
+  const int64_t* labels;          /* host [z][y][x]; ids <= 0 are background */
+  int32_t image_shape_zyx[3];
+  int32_t label_shape_zyx[3];
+  float offset, scale;            /* image normalisation of this volume */
+} FfnExampleVolume;
+typedef struct {
+  int32_t policy;                 /* FFN_FOV_* */
+  int32_t fov_moves;              /* >= 1 */
+  float seed_pad;                 /* in (0, 1) */
+  float seed_logit_pad;           /* float32 logit(seed_pad) and logit(0.95) of the fresh seed, as the host computes */
+  float seed_logit_centre;        /*   them (scipy.special.logit on float32) */
+  int32_t batch;
+  double seed_threshold;          /* logit(threshold): a move's target is valid when seed >= it, compared in float64 */
+  double label_threshold;         /* expit(logit(threshold)): wanted when label >= it (max_pred_moves), in float64 */
+  const int32_t* shifts_zyx;      /* fixed: [n_shifts][3], the visiting order after the centre */
+  int32_t n_shifts;
+  int32_t permutable_zyx[3];      /* nonzero: the axis may be permuted (all such axes need equal patch extents) */
+  int32_t reflectable_zyx[3];     /* nonzero: the axis may be reflected */
+} FfnExampleDesc;
+/* model: the fov and deltas of the network trained (the trainer's).  The volumes are copied to the device.  Fails
+ * for seed_pad outside (0, 1), a fresh seed whose centre fails seed_threshold, permutable axes of unequal patch extent,
+ * a batch outside [1, 32], fov_moves < 1 or patches of 2^31 or more voxels.  The object owns all its device memory. */
+int ffn_examples_create(int device, const FfnModelDesc* model, const FfnExampleDesc* desc,
+                        const FfnExampleVolume* volumes, int n_volumes, FfnExamples** out);
+void ffn_examples_destroy(FfnExamples* examples);
+/* One step of the loop without training: coords are the next n_coords entries of the example stream (at least
+ * batch).  Writes the batch (seed, image, labels: host float32 [batch, Z, Y, X]; any may be NULL), each element's
+ * offset (z, y, x) from its patch centre and index of its example in the stream since creation, and the entries
+ * taken.  Fails, changing nothing, for a coordinate whose crop leaves its volume, an unknown volume or a permutation or
+ * reflection of an axis the description does not allow. */
+int ffn_examples_next(FfnExamples* examples, const FfnExampleCoord* coords, int64_t n_coords, float* seed_out,
+                      float* image_out, float* labels_out, int32_t* offsets_zyx_out, int64_t* example_out,
+                      int64_t* n_consumed);
+/* Pastes logits (host float32 [batch, Z, Y, X]) into each element's seed at its current offset. */
+int ffn_examples_update(FfnExamples* examples, const float* logits);
+/* The seed canvases, host float32 [batch, patch z, y, x]. */
+int ffn_examples_read_seeds(FfnExamples* examples, float* out);
+/* n_steps training steps fed by the example loop, with no host copy and one host synchronisation: per step the loop's
+ * next batch, ffn_trainer_step's step at learning_rate[i] with unit loss weights, and the logits pasted back.
+ * losses_out[i] equals ffn_trainer_step's loss bit for bit.  coords: at least n_steps * batch stream entries;
+ * *n_consumed: the entries taken.  Fails for examples of another fov or a batch above the trainer's max_batch. */
+int ffn_trainer_train(FfnTrainer* trainer, FfnExamples* examples, const FfnExampleCoord* coords, int64_t n_coords,
+                      int n_steps, const float* learning_rate, double* losses_out, int64_t* n_consumed);
+
 /* Known-answer test of the wgmma descriptors (worst absolute error of each case in out[]; see
  * ffn_selftest_wgmma in ffn_b200/csrc/engine.cu).  Used by tests, not by the product path. */
 int ffn_selftest_wgmma(int device, double* out, int n_out);
