@@ -38,7 +38,8 @@ EXPORTS = [
     'ffn_canvas_add_id_offset', 'ffn_decision_points', 'ffn_reseg_eval', 'ffn_split_intersection', 'ffn_compute_partitions',
     'ffn_partition_rows', 'ffn_coordinate_records', 'ffn_clean_up', 'ffn_trainer_create', 'ffn_trainer_destroy',
     'ffn_trainer_step', 'ffn_trainer_gradients', 'ffn_trainer_get_weights', 'ffn_trainer_train', 'ffn_examples_create',
-    'ffn_examples_destroy', 'ffn_examples_next', 'ffn_examples_update', 'ffn_examples_read_seeds', 'ffn_selftest_wgmma',
+    'ffn_examples_destroy', 'ffn_examples_next', 'ffn_examples_update', 'ffn_examples_read_seeds', 'ffn_examples_tracker',
+    'ffn_selftest_wgmma',
 ]
 
 
@@ -118,7 +119,12 @@ class ExampleDesc(C.Structure):
   _fields_ = [('policy', C.c_int32), ('fov_moves', C.c_int32), ('seed_pad', C.c_float), ('seed_logit_pad', C.c_float),
               ('seed_logit_centre', C.c_float), ('batch', C.c_int32), ('seed_threshold', C.c_double),
               ('label_threshold', C.c_double), ('shifts_zyx', C.c_void_p), ('n_shifts', C.c_int32),
-              ('permutable_zyx', C.c_int32 * 3), ('reflectable_zyx', C.c_int32 * 3)]
+              ('permutable_zyx', C.c_int32 * 3), ('reflectable_zyx', C.c_int32 * 3), ('eval_threshold', C.c_double)]
+
+
+class TrackerCounts(C.Structure):
+  _fields_ = [('steps', C.c_int64), ('patches', C.c_int64), ('eval_voxels', C.c_int64),
+              ('prediction_counts', C.c_int64 * 4), ('patch_loss', C.c_double)]
 
 
 class CleanUpDesc(C.Structure):
@@ -245,6 +251,7 @@ def load() -> C.CDLL:
   lib.ffn_examples_next.argtypes = [p, p, C.c_int64, p, p, p, p, p, C.POINTER(C.c_int64)]
   lib.ffn_examples_update.argtypes = [p, p]
   lib.ffn_examples_read_seeds.argtypes = [p, p]
+  lib.ffn_examples_tracker.argtypes = [p, C.POINTER(TrackerCounts), p, C.c_int, p, p, C.POINTER(C.c_int32), C.c_int]
   lib.ffn_selftest_wgmma.argtypes = [C.c_int, C.POINTER(C.c_double), C.c_int]
   for name in EXPORTS:
     if name not in ('ffn_last_error', 'ffn_engine_destroy', 'ffn_canvas_destroy', 'ffn_trainer_destroy',

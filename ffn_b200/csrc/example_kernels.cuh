@@ -12,6 +12,11 @@ namespace exk {
 constexpr int kThreads = 256;
 constexpr int kMaxWarps = 32;   // the resume kernel runs one warp per element, in one CTA
 
+constexpr int kRing = 16;      // finished examples whose centre planes the tracker keeps (EvalTracker's deques)
+
+// Tracker counters, int64 slots of Args::tk; the moves follow as [radius][MoveType] (CORRECT, MISSED, SPURIOUS).
+enum { kTkSteps, kTkPatches, kTkVoxels, kTkTP, kTkTN, kTkFP, kTkFN, kTkRing, kTkMoves };
+
 // One element's generator state.  `off` is the offset of the last yield; fixed resumes at shift k (0: the centre),
 // max_pred_moves pops queue[head .. tail) after extending it from the seed at `off`.
 struct State {
@@ -48,7 +53,34 @@ struct Args {
   int* entry;                       // [batch]: the entry an element loads this step, or -1
   long long* total;                 // examples loaded since creation
   int* error;                       // set when a queue would overflow its bound (never, by construction)
+  // EvalTracker (ffn/training/tracker.py) of the finished examples: eval crop E (fov + 2 * deltas * fov_moves,
+  // centred in the patch at ecrop), float64 eval threshold logit(0.9)
+  int E[3], ecrop[3];
+  long long EV;
+  int tk_blocks;                    // blocks per element of `track`
+  double eval_thr;
+  const int* shift_r;               // [n_shifts]: int(norm(shift)), the radius its moves are counted at
+  long long* tk;                    // kTk* counters, then moves [n_radii][3]
+  double* tk_loss;                  // sum of the finished patches' mean losses
+  double* tk_part;                  // [batch][tk_blocks] per-block loss sums of the current step
+  unsigned* tk_arrived;             // [2]: blocks of `track` done this step, and expected (the last adds the sums)
+  int* tk_slot;                     // [batch]: ring slot of the element's example finished this step; -2: finished
+                                    //   but not kept (a later one of the step takes the slot); -1: not finished
+  FfnExampleCoord* ecoord;          // [batch]: the stream entry of each element's current example
+  float* ring;                      // [kRing][plane_floats()]: labels and logits of the xy, xz and yz centre planes
+  FfnExampleCoord* ring_coord;      // [kRing]
 };
+
+__host__ __device__ inline long long plane_floats(const int E[3]) {
+  return 2ll * ((long long)E[1] * E[2] + (long long)E[0] * E[2] + (long long)E[0] * E[1]);
+}
+
+// EvalTracker.record_move: CORRECT when wanted and executed, MISSED when wanted only, SPURIOUS when executed only.
+__device__ __forceinline__ void record_move(const Args& a, int r, bool wanted, bool executed) {
+  if (!wanted && !executed) return;
+  const int t = wanted ? (executed ? 0 : 1) : 2;
+  atomicAdd((unsigned long long*)&a.tk[kTkMoves + r * 3 + t], 1ull);
+}
 
 __device__ __forceinline__ int floor_div(int a, int b) { return a >= 0 ? a / b : -((-a + b - 1) / b); }
 
@@ -73,13 +105,16 @@ __device__ __forceinline__ bool before(float s, const int* p, float t, const int
 
 // Fixed policy (examples.fixed_offsets): the centre, then the shifts in order, each yielded when the seed at it
 // passes the threshold.  Returns 1 when exhausted.  One thread.
-__device__ int resume_fixed(const Args& a, State& s, const float* seed) {
+__device__ int resume_fixed(const Args& a, State& s, const float* seed, const float* labels) {
   const int c[3] = {a.S[0] / 2, a.S[1] / 2, a.S[2] / 2};
   for (int k = s.k; k <= a.n_shifts; ++k) {
     int o[3] = {0, 0, 0};
     if (k > 0)
       for (int d = 0; d < 3; ++d) o[d] = a.shifts[(k - 1) * 3 + d];
-    if ((double)seed[at(a, c[0] + o[0], c[1] + o[1], c[2] + o[2])] >= a.seed_thr) {
+    const long long v = at(a, c[0] + o[0], c[1] + o[1], c[2] + o[2]);
+    const bool valid = (double)seed[v] >= a.seed_thr;
+    record_move(a, k > 0 ? a.shift_r[k - 1] : 0, (double)labels[v] >= a.label_thr, valid);
+    if (valid) {
       for (int d = 0; d < 3; ++d) s.off[d] = o[d];
       s.k = k + 1;
       return 0;
@@ -91,7 +126,8 @@ __device__ int resume_fixed(const Args& a, State& s, const float* seed) {
 
 // max_pred_moves (examples.max_pred_offsets): extend the queue with movement.get_scored_move_offsets of the seed at
 // the last yield, sorted in reverse, then pop until an offset inside max_radius, in an unvisited quantised cell,
-// valid, and wanted unless it is the centre.  One warp; returns 1 (to every lane) when exhausted.
+// valid, and wanted unless it is the centre.  Every popped entry inside max_radius and unvisited is a move, recorded
+// at radius 0 as the reference records it.  One warp; returns 1 (to every lane) when exhausted.
 __device__ int resume_max_pred(const Args& a, State& s, int e, const float* seed, const float* labels, int lane) {
   const int c[3] = {a.S[0] / 2, a.S[1] / 2, a.S[2] / 2};
   int* q = a.queue + (size_t)e * a.qcap * 3;
@@ -163,6 +199,7 @@ __device__ int resume_max_pred(const Args& a, State& s, int e, const float* seed
       const long long v = at(a, c[0] + o[0], c[1] + o[1], c[2] + o[2]);
       const bool valid = (double)seed[v] >= a.seed_thr;
       const bool wanted = (double)labels[v] >= a.label_thr;
+      record_move(a, 0, wanted, valid);
       if (!valid || (!wanted && !centre)) continue;
       *done = 1;
       for (int d = 0; d < 3; ++d) s.off[d] = o[d];
@@ -174,7 +211,7 @@ __device__ int resume_max_pred(const Args& a, State& s, int e, const float* seed
 }
 
 // Resumes every element's generator (one warp each), then hands the next stream entries to the exhausted elements
-// in element order.
+// in element order, and gives the finished examples among them their ring slots, in the same order.
 __global__ void __launch_bounds__(kMaxWarps * 32) resume(Args a) {
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32, nw = blockDim.x / 32;
   for (int e = warp; e < a.batch; e += nw) {
@@ -183,7 +220,7 @@ __global__ void __launch_bounds__(kMaxWarps * 32) resume(Args a) {
     if (s.active) {
       const float* seed = a.seed + e * a.SV;
       if (a.policy == FFN_FOV_FIXED) {
-        if (lane == 0) need = resume_fixed(a, s, seed);
+        if (lane == 0) need = resume_fixed(a, s, seed, a.labels + e * a.SV);
       } else {
         need = resume_max_pred(a, s, e, seed, a.labels + e * a.SV, lane);
       }
@@ -192,17 +229,104 @@ __global__ void __launch_bounds__(kMaxWarps * 32) resume(Args a) {
   }
   __syncthreads();
   if (threadIdx.x == 0) {
+    long long* tk = a.tk;
     for (int e = 0; e < a.batch; ++e) {
+      a.tk_slot[e] = -1;
       if (a.entry[e] < 0) continue;
       a.entry[e] = (*a.used)++;
+      if (a.st[e].active) {
+        a.tk_slot[e] = (int)(tk[kTkRing]++ % kRing);
+        tk[kTkPatches] += 1;
+        tk[kTkVoxels] += a.EV;
+      }
       a.st[e].example = (*a.total)++;
     }
+    // more finished examples than ring slots in one step: the ring keeps the last kRing of them
+    int n = 0;
+    for (int e = a.batch - 1; e >= 0; --e)
+      if (a.tk_slot[e] >= 0 && ++n > kRing) a.tk_slot[e] = -2;
+    a.tk_arrived[1] = n * a.tk_blocks;
+    tk[kTkSteps] += 1;
   }
+}
+
+// EvalTracker.add_patch of every example `resume` found finished: on the eval crop of its seed (logits) and labels,
+// TP / TN / FP / FN of (seed >= logit(0.9), label > 0.5), the mean sigmoid cross-entropy in float64, and the three
+// centre planes into its ring slot.  Per-block loss sums go to fixed slots and the last block to arrive adds them up
+// in a fixed order (a fixed tree per example, then the examples in element order), so the loss does not depend on
+// the blocks' timing.  The blocks of unfinished elements return at once.  grid (tk_blocks, batch).
+__global__ void __launch_bounds__(kThreads) track(Args a) {
+  const int e = blockIdx.y, slot = a.tk_slot[e];
+  __shared__ double red[kThreads];
+  __shared__ unsigned long long cnt[4];
+  __shared__ bool last;
+  if (slot == -1) return;
+  if (threadIdx.x < 4) cnt[threadIdx.x] = 0;
+  __syncthreads();
+  const float* seed = a.seed + e * a.SV;
+  const float* labels = a.labels + e * a.SV;
+  float* ring = slot >= 0 ? a.ring + slot * plane_floats(a.E) : nullptr;
+  const long long pxy = (long long)a.E[1] * a.E[2], pxz = (long long)a.E[0] * a.E[2];
+  double sum = 0.0;
+  unsigned c[4] = {0, 0, 0, 0};
+  for (long long v = blockIdx.x * (long long)blockDim.x + threadIdx.x; v < a.EV; v += (long long)gridDim.x * blockDim.x) {
+    const int x = (int)(v % a.E[2]), y = (int)(v / a.E[2] % a.E[1]), z = (int)(v / ((long long)a.E[2] * a.E[1]));
+    const long long src = at(a, a.ecrop[0] + z, a.ecrop[1] + y, a.ecrop[2] + x);
+    const float lg = seed[src], lb = labels[src];
+    const bool pred = (double)lg >= a.eval_thr, truth = lb > 0.5f;
+    c[0] += pred && truth;   // TP, TN, FP, FN
+    c[1] += !pred && !truth;
+    c[2] += pred && !truth;
+    c[3] += !pred && truth;
+    const double xd = lg, zd = lb;
+    sum += (fmax(xd, 0.0) - xd * zd) + log1p(exp(-fabs(xd)));
+    if (!ring) continue;
+    if (z == a.E[0] / 2) ring[(long long)y * a.E[2] + x] = lb, ring[pxy + (long long)y * a.E[2] + x] = lg;
+    if (y == a.E[1] / 2) ring[2 * pxy + (long long)z * a.E[2] + x] = lb, ring[2 * pxy + pxz + (long long)z * a.E[2] + x] = lg;
+    if (x == a.E[2] / 2) {
+      const long long b = 2 * (pxy + pxz);
+      ring[b + (long long)z * a.E[1] + y] = lb;
+      ring[b + (long long)a.E[0] * a.E[1] + (long long)z * a.E[1] + y] = lg;
+    }
+  }
+  for (int k = 0; k < 4; ++k)
+    if (c[k]) atomicAdd(&cnt[k], (unsigned long long)c[k]);
+  red[threadIdx.x] = sum;
+  __syncthreads();
+  for (int m = kThreads / 2; m; m >>= 1) {
+    if (threadIdx.x < m) red[threadIdx.x] += red[threadIdx.x + m];
+    __syncthreads();
+  }
+  if (threadIdx.x < 4) atomicAdd((unsigned long long*)&a.tk[kTkTP + threadIdx.x], cnt[threadIdx.x]);
+  if (threadIdx.x == 0) {
+    a.tk_part[e * a.tk_blocks + blockIdx.x] = red[0];
+    if (blockIdx.x == 0 && slot >= 0) a.ring_coord[slot] = a.ecoord[e];
+  }
+  if (threadIdx.x == 0) {
+    __threadfence();
+    last = atomicAdd(a.tk_arrived, 1u) == a.tk_arrived[1] - 1;
+  }
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  for (int f = 0; f < a.batch; ++f) {   // tk_blocks <= kThreads
+    if (a.tk_slot[f] == -1) continue;
+    red[threadIdx.x] = threadIdx.x < a.tk_blocks ? __ldcg(a.tk_part + f * a.tk_blocks + threadIdx.x) : 0.0;
+    __syncthreads();
+    for (int m = kThreads / 2; m; m >>= 1) {
+      if (threadIdx.x < m) red[threadIdx.x] += red[threadIdx.x + m];
+      __syncthreads();
+    }
+    if (threadIdx.x == 0) *a.tk_loss += red[0] / (double)a.EV;
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) a.tk_arrived[0] = 0;
 }
 
 // Loads the examples handed out by `resume` (inputs.load_from_numpylike, the object mask of the centre label,
 // soften_labels, PermuteAndReflect, offset_and_scale_patches) and starts their generators at the centre, which a
-// fresh seed always passes.  grid (blocks, batch).
+// fresh seed always passes; that first move is recorded here (radius 0, wanted by the centre's soft label), as both
+// policies record it when the reference starts their generator.  grid (blocks, batch).
 __global__ void __launch_bounds__(kThreads) load(Args a) {
   const int e = blockIdx.y;
   const int j = a.entry[e];
@@ -223,6 +347,7 @@ __global__ void __launch_bounds__(kThreads) load(Args a) {
       s.head = s.tail = 0;
       s.active = 1;
       done[(a.moves * a.side + a.moves) * a.side + a.moves] = 1;
+      a.ecoord[e] = cd;
     }
   }
   auto lab_at = [&](int z, int y, int x) {
@@ -244,7 +369,9 @@ __global__ void __launch_bounds__(kThreads) load(Args a) {
     labels[v] = l > 0 && l == centre ? 0.95f : 0.05f;
     const uint8_t u = vol.image[((long long)src[0] * vol.ishape[1] + src[1]) * vol.ishape[2] + src[2]];
     image[v] = __fdiv_rn(__fsub_rn((float)u, vol.offset), vol.scale);
-    seed[v] = o[0] == a.S[0] / 2 && o[1] == a.S[1] / 2 && o[2] == a.S[2] / 2 ? a.centre_logit : a.pad_logit;
+    const bool at_centre = o[0] == a.S[0] / 2 && o[1] == a.S[1] / 2 && o[2] == a.S[2] / 2;
+    seed[v] = at_centre ? a.centre_logit : a.pad_logit;
+    if (at_centre) record_move(a, 0, (double)labels[v] >= a.label_thr, (double)a.centre_logit >= a.seed_thr);
   }
 }
 

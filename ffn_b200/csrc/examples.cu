@@ -22,6 +22,7 @@ struct FfnExamples {
   FfnExampleCoord* coords = nullptr;
   float *bseed = nullptr, *bimage = nullptr, *blabels = nullptr, *logits = nullptr;
   int64_t total = 0;                    // examples loaded since creation, as of the last call
+  int n_radii = 1;                      // moves are counted at radii 0 .. n_radii - 1
   ~FfnExamples() {
     cudaSetDevice(device);
     cudaDeviceSynchronize();
@@ -92,12 +93,14 @@ int examples_upload(FfnExamples* ex, const FfnExampleCoord* coords, int64_t n) {
   return 0;
 }
 
-// One step's batch: resume every generator, load the exhausted elements' next examples, crop [batch][F] into the
+// One step's batch: resume every generator, track the examples it finished, load the exhausted elements' next examples, crop [batch][F] into the
 // three outputs (device pointers).
 int examples_advance(FfnExamples* ex, float* seed, float* image, float* labels) {
   cudaStream_t st = cudaStreamPerThread;
   const exk::Args& a = ex->a;
   exk::resume<<<1, 32 * std::min(a.batch, exk::kMaxWarps), 0, st>>>(a);
+  CUDA_OK(cudaGetLastError());
+  exk::track<<<dim3(a.tk_blocks, a.batch), exk::kThreads, 0, st>>>(a);
   CUDA_OK(cudaGetLastError());
   exk::load<<<dim3(grid_blocks(a.SV), a.batch), exk::kThreads, 0, st>>>(a);
   CUDA_OK(cudaGetLastError());
@@ -146,6 +149,7 @@ int ffn_examples_create(int device, const FfnModelDesc* model, const FfnExampleD
     return fail("batch must lie in [1, " + std::to_string(exk::kMaxWarps) + "]");
   if (desc->policy == FFN_FOV_FIXED && desc->n_shifts > 0 && !desc->shifts_zyx) return fail("null shifts");
   if (desc->n_shifts < 0) return fail("negative n_shifts");
+  if (!std::isfinite(desc->eval_threshold)) return fail("eval_threshold must be finite");
 
   std::unique_ptr<FfnExamples> ex(new FfnExamples());
   exk::Args& a = ex->a;
@@ -182,6 +186,21 @@ int ffn_examples_create(int device, const FfnModelDesc* model, const FfnExampleD
   a.seed_thr = desc->seed_threshold;
   a.label_thr = desc->label_threshold;
   a.n_shifts = desc->policy == FFN_FOV_FIXED ? desc->n_shifts : 0;
+  a.eval_thr = desc->eval_threshold;
+  a.EV = 1;
+  for (int d = 0; d < 3; ++d) {
+    a.E[d] = a.F[d] + 2 * a.D[d] * desc->fov_moves;   // train.py's train_eval_size
+    a.ecrop[d] = a.S[d] / 2 - a.E[d] / 2;             // mask.crop_and_pad(..., (0, 0, 0), E)
+    a.EV *= a.E[d];
+  }
+  a.tk_blocks = grid_blocks(a.EV);
+  // EvalTracker.record_move's radius, int(np.linalg.norm(shift)): the square root of an exact integer, truncated
+  std::vector<int> shift_r(std::max(a.n_shifts, 1), 0);
+  for (int i = 0; i < a.n_shifts; ++i) {
+    const int* o = desc->shifts_zyx + i * 3;
+    shift_r[i] = (int)std::sqrt((double)o[0] * o[0] + (double)o[1] * o[1] + (double)o[2] * o[2]);
+    ex->n_radii = std::max(ex->n_radii, shift_r[i] + 1);
+  }
   ex->desc = *desc;
   ex->desc.shifts_zyx = nullptr;
   ex->n_volumes = n_volumes;
@@ -218,6 +237,14 @@ int ffn_examples_create(int device, const FfnModelDesc* model, const FfnExampleD
   exk::Vol* vd = nullptr;
   int* shifts = nullptr;
   const size_t B = a.batch;
+  int* sr = nullptr;
+  if (m.get(&sr, shift_r.size()) || m.get(&a.tk, exk::kTkMoves + 3 * ex->n_radii, true) ||
+      m.get(&a.tk_loss, 1, true) || m.get(&a.tk_part, B * a.tk_blocks, true) || m.get(&a.tk_arrived, 2, true) ||
+      m.get(&a.tk_slot, B, true) || m.get(&a.ecoord, B, true) || m.get(&a.ring, exk::kRing * exk::plane_floats(a.E), true) ||
+      m.get(&a.ring_coord, exk::kRing, true))
+    return 1;
+  CUDA_OK(cudaMemcpy(sr, shift_r.data(), shift_r.size() * sizeof(int), cudaMemcpyHostToDevice));
+  a.shift_r = sr;
   if (m.get(&vd, n_volumes) || m.get(&shifts, std::max(a.n_shifts, 1) * 3) || m.get(&a.seed, B * a.SV, true) ||
       m.get(&a.image, B * a.SV, true) || m.get(&a.labels, B * a.SV, true) || m.get(&a.st, B, true) ||
       m.get(&a.queue, B * a.qcap * 3, true) || m.get(&a.done, B * a.side * a.side * a.side, true) ||
@@ -277,6 +304,48 @@ int ffn_examples_read_seeds(FfnExamples* ex, float* out) {
   CUDA_OK(cudaMemcpyAsync(out, ex->a.seed, (size_t)ex->a.batch * ex->a.SV * 4, cudaMemcpyDeviceToHost,
                           cudaStreamPerThread));
   CUDA_OK(cudaStreamSynchronize(cudaStreamPerThread));
+  return 0;
+}
+
+int ffn_examples_tracker(FfnExamples* ex, FfnTrackerCounts* out, int64_t* moves_by_radius, int n_radii,
+                         float* planes, FfnExampleCoord* plane_coords, int32_t* n_planes, int reset) {
+  if (!ex) return fail("null examples");
+  if (!out || !moves_by_radius || !n_planes) return fail("null argument: counts, moves_by_radius and n_planes are required");
+  if (n_radii < ex->n_radii)
+    return fail("moves_by_radius holds " + std::to_string(n_radii) + " radii, the shifts need " +
+                std::to_string(ex->n_radii));
+  if (!planes != !plane_coords) return fail("planes and plane_coords must both be given or both be NULL");
+  CUDA_OK(cudaSetDevice(ex->device));
+  cudaStream_t st = cudaStreamPerThread;
+  const exk::Args& a = ex->a;
+  std::vector<long long> tk(exk::kTkMoves + 3 * ex->n_radii);
+  double loss = 0.0;
+  CUDA_OK(cudaMemcpyAsync(tk.data(), a.tk, tk.size() * sizeof(long long), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaMemcpyAsync(&loss, a.tk_loss, sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+  const int n = (int)std::min<long long>(tk[exk::kTkRing], exk::kRing);
+  if (planes) {
+    const long long pf = exk::plane_floats(a.E);
+    for (int i = 0; i < n; ++i) {   // oldest first
+      const int slot = (int)((tk[exk::kTkRing] - n + i) % exk::kRing);
+      CUDA_OK(cudaMemcpyAsync(planes + i * pf, a.ring + slot * pf, pf * sizeof(float), cudaMemcpyDeviceToHost, st));
+      CUDA_OK(cudaMemcpyAsync(plane_coords + i, a.ring_coord + slot, sizeof(FfnExampleCoord), cudaMemcpyDeviceToHost,
+                              st));
+    }
+  }
+  if (reset) {
+    CUDA_OK(cudaMemsetAsync(a.tk, 0, tk.size() * sizeof(long long), st));
+    CUDA_OK(cudaMemsetAsync(a.tk_loss, 0, sizeof(double), st));
+  }
+  CUDA_OK(cudaStreamSynchronize(st));
+  out->steps = tk[exk::kTkSteps];
+  out->patches = tk[exk::kTkPatches];
+  out->eval_voxels = tk[exk::kTkVoxels];
+  for (int k = 0; k < 4; ++k) out->prediction_counts[k] = tk[exk::kTkTP + k];
+  out->patch_loss = loss;
+  for (int r = 0; r < n_radii; ++r)
+    for (int t = 0; t < 3; ++t) moves_by_radius[r * 3 + t] = r < ex->n_radii ? tk[exk::kTkMoves + r * 3 + t] : 0;
+  *n_planes = n;
   return 0;
 }
 

@@ -22,6 +22,7 @@ import numpy as np
 from scipy import special
 
 from .. import _lib
+from . import tracker as _tracker
 
 LABEL_SOFT_TRUE = np.float32(0.95)
 
@@ -162,7 +163,8 @@ class ExampleLoop:
     desc = _lib.ExampleDesc(policy=_lib.FOV_POLICIES[fov_policy], fov_moves=int(fov_moves), seed_pad=float(seed_pad),
                             seed_logit_pad=float(pad_logit), seed_logit_centre=float(centre_logit),
                             batch=self.batch_size, seed_threshold=seed_thr, label_threshold=label_thr,
-                            shifts_zyx=shifts.ctypes.data, n_shifts=len(shifts))
+                            shifts_zyx=shifts.ctypes.data, n_shifts=len(shifts),
+                            eval_threshold=float(_tracker.EVAL_THRESHOLD))
     perm = set(int(a) for a in stream.permutable)
     refl = set(int(a) for a in stream.reflectable)
     desc.permutable_zyx = _lib.i3([int(a in perm) for a in range(3)])
@@ -172,6 +174,9 @@ class ExampleLoop:
     model.deltas_zyx = _lib.i3(self.deltas_zyx)
     model.depth = 1
     model.features = 32
+    self.eval_zyx = _tracker.eval_shape(self.fov_zyx, self.deltas_zyx, fov_moves)
+    # EvalTracker's radii come from model.shifts; the fixed policy's own shifts may add more
+    self.radii = _tracker.radii(model_shifts(self.deltas_zyx) + (shifts.tolist() if fov_policy == 'fixed' else []))
     h = C.c_void_p()
     _lib.check(self._lib.ffn_examples_create(int(device), C.byref(model), C.byref(desc), C.cast(vol_arr, C.c_void_p),
                                              len(vols), C.byref(h)))
@@ -228,3 +233,25 @@ class ExampleLoop:
     out = np.empty((self.batch_size,) + self.patch_zyx, np.float32)
     _lib.check(self._lib.ffn_examples_read_seeds(self.handle, _lib.ptr(out)))
     return out
+
+  def tracker(self, reset: bool = False) -> _tracker.TrackerState:
+    """The tracker's counts since the last reset and the planes of the last (up to 16) finished examples, oldest
+    first; reset: then zero the counts and empty the ring, as EvalTracker.reset() after get_summaries()."""
+    counts = _lib.TrackerCounts()
+    n_r = max(self.radii) + 1
+    moves = np.zeros((n_r, 3), np.int64)
+    pf = 2 * (self.eval_zyx[1] * self.eval_zyx[2] + self.eval_zyx[0] * self.eval_zyx[2] +
+              self.eval_zyx[0] * self.eval_zyx[1])
+    planes = np.zeros((_tracker.RING, pf), np.float32)
+    coords = np.zeros(_tracker.RING, _lib.EXAMPLE_COORD_DTYPE)
+    n = C.c_int32()
+    _lib.check(self._lib.ffn_examples_tracker(self.handle, C.byref(counts), _lib.ptr(moves), n_r, _lib.ptr(planes),
+                                              _lib.ptr(coords), C.byref(n), int(bool(reset))))
+    k = n.value
+    return _tracker.TrackerState(
+        steps=counts.steps, fov_voxels=counts.steps * self.batch_size * int(np.prod(self.fov_zyx)),
+        patches=counts.patches, eval_voxels=counts.eval_voxels,
+        prediction_counts=np.array(counts.prediction_counts[:], np.int64), patch_loss=counts.patch_loss,
+        moves={r: moves[r].copy() for r in self.radii},
+        planes=[_tracker.split_planes(planes[i], self.eval_zyx) for i in range(k)],
+        coords=[(int(c['volume']), tuple(int(v) for v in c['center_xyz'])) for c in coords[:k]])

@@ -517,6 +517,7 @@ typedef struct {
   int32_t n_shifts;
   int32_t permutable_zyx[3];      /* nonzero: the axis may be permuted (all such axes need equal patch extents) */
   int32_t reflectable_zyx[3];     /* nonzero: the axis may be reflected */
+  double eval_threshold;          /* the tracker's logit(0.9) (scipy's value): a voxel is predicted when seed >= it */
 } FfnExampleDesc;
 /* model: the fov and deltas of the network trained (the trainer's).  The volumes are copied to the device.  Fails
  * for seed_pad outside (0, 1), a fresh seed whose centre fails seed_threshold, permutable axes of unequal patch extent,
@@ -536,6 +537,26 @@ int ffn_examples_next(FfnExamples* examples, const FfnExampleCoord* coords, int6
 int ffn_examples_update(FfnExamples* examples, const float* logits);
 /* The seed canvases, host float32 [batch, patch z, y, x]. */
 int ffn_examples_read_seeds(FfnExamples* examples, float* out);
+/* The tracker of the loop (ffn/training/tracker.py's EvalTracker, as examples.py feeds it), kept on the device by
+ * every step of ffn_examples_next and ffn_trainer_train.  Moves: every move the policy evaluates, as record_move
+ * counts them, at radius int(|shift|) for fixed and 0 for max_pred_moves; the centre move of each new example counts.
+ * Finished examples (add_patch): on the crop of fov + 2 * deltas * fov_moves voxels at the patch centre, TP / TN /
+ * FP / FN of (seed >= eval_threshold, label > 0.5) and the mean sigmoid cross-entropy
+ * max(x, 0) - x z + log1p(exp(-|x|)) in float64, and the centre planes of the last 16 of them. */
+typedef struct {
+  int64_t steps;                  /* loop steps */
+  int64_t patches;                /* finished examples */
+  int64_t eval_voxels;            /* voxels of their eval crops */
+  int64_t prediction_counts[4];   /* TP, TN, FP, FN */
+  double patch_loss;              /* sum of the finished examples' mean losses, in finishing order */
+} FfnTrackerCounts;
+/* Reads the counts since the last reset.  moves_by_radius: [n_radii][3] (correct, missed, spurious) at radius
+ * 0 .. n_radii - 1; n_radii must cover every shift's radius.  planes (float32) and plane_coords: NULL, or room for 16
+ * finished examples, oldest first, each [xy labels, xy logits, xz labels, xz logits, yz labels, yz logits] of the crop
+ * E (zyx) at z = E0 / 2, y = E1 / 2 and x = E2 / 2 ([E1][E2], [E0][E2], [E0][E1] each), with its stream entry;
+ * *n_planes: how many.  reset: then zero the counts and empty the ring (examples in flight are not touched). */
+int ffn_examples_tracker(FfnExamples* examples, FfnTrackerCounts* out, int64_t* moves_by_radius, int n_radii,
+                         float* planes, FfnExampleCoord* plane_coords, int32_t* n_planes, int reset);
 /* n_steps training steps fed by the example loop, with no host copy and one host synchronisation: per step the loop's
  * next batch, ffn_trainer_step's step at learning_rate[i] with unit loss weights, and the logits pasted back.
  * losses_out[i] equals ffn_trainer_step's loss bit for bit.  coords: at least n_steps * batch stream entries;

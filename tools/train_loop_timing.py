@@ -6,8 +6,8 @@ host batches, at the FIB-25 geometry (33^3 field of view, depth 12, deltas 8, ba
 Each repeat times --steps steps with a host clock around calls that end in a device synchronisation, after a warm-up;
 the median and the spread over --reps repeats are reported for both policies (fixed, max_pred_moves) and for
 Trainer.step on batches the loop produced beforehand (no loop work between steps, but the host copies step() makes).
---profile instead records Trainer.train with torch.profiler and reports the example-loop kernels' device time per step
-(run it as a separate command).  One JSON line on stdout (and in DIR), with the GPU's name and power limit read in the
+--profile instead records Trainer.train with torch.profiler and reports the example-loop kernels' device time per step,
+and the tracker's `track` kernel's on its own (run it as a separate command).  One JSON line on stdout (and in DIR), with the GPU's name and power limit read in the
 same run.
 """
 
@@ -23,7 +23,7 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 
 FOV, DELTAS, BATCH = (33, 33, 33), (8, 8, 8), 4
-LOOP_KERNELS = ('exk::resume', 'exk::load', 'exk::crop', 'exk::paste', 'sum_loss')
+LOOP_KERNELS = ('exk::resume', 'exk::track', 'exk::load', 'exk::crop', 'exk::paste', 'sum_loss')
 
 
 def _gpu():
@@ -89,7 +89,7 @@ def profile(args):
     trainer.train(loop, 10)
     with torch.profiler.profile(activities=[ProfilerActivity.CUDA]) as prof:
       trainer.train(loop, args.steps)
-    loop_us = total_us = 0.0
+    loop_us = total_us = track_us = 0.0
     for ev in prof.key_averages():
       t = getattr(ev, 'device_time_total', None)
       if t is None:
@@ -97,7 +97,10 @@ def profile(args):
       total_us += t
       if any(k in ev.key for k in LOOP_KERNELS):
         loop_us += t
-    out[policy] = {'loop_kernels_us_per_step': loop_us / args.steps, 'all_kernels_us_per_step': total_us / args.steps}
+      if 'exk::track' in ev.key:
+        track_us += t
+    out[policy] = {'loop_kernels_us_per_step': loop_us / args.steps, 'all_kernels_us_per_step': total_us / args.steps,
+                   'track_us_per_step': track_us / args.steps}
     loop.close()
     trainer.close()
   return out

@@ -19,8 +19,12 @@ ffn_b200.training.trainer).  Differences from the reference script:
     own, so the weights are not correlated with the data order);
   * checkpoints are `model.ckpt-<step>.npz` files of w00.. / b00.. arrays (what ffn_b200/tf_checkpoint.py and
     run_inference.py read), written every 300 s and at the end; a run does not resume from them;
-  * the loss is logged every `--summary_rate_secs`; there are no TF summaries, and `fixed_offsets_window`,
-    `no_step`, multichannel volumes and several replicas are not supported.
+  * every `--summary_rate_secs`, at the first boundary of a call of STEPS_PER_CALL steps after that time, the loss
+    is logged and the EvalTracker summaries (moves, the final object masks' loss and prediction metrics, their
+    centre slices; ffn_b200.training.tracker), with pixel_loss, optimizer_loss and learning_rate, are appended to a
+    TensorBoard event file in `--train_dir`, and the tracker is reset.  The tracker runs on the device with the
+    example loop; the weight and gradient histograms are not written;
+  * `fixed_offsets_window`, `no_step`, multichannel volumes and several replicas are not supported.
 `<path>:<dataset>` volumes are read with h5py when it is installed, otherwise from `.npy` (`file.npy:`) or `.npz`
 (`file.npz:key`) files.
 """
@@ -37,6 +41,8 @@ from absl import flags
 
 from ffn_b200.training import examples as ex
 from ffn_b200.training import inputs
+from ffn_b200.training import summary
+from ffn_b200.training import tracker
 from ffn_b200.training.trainer import Trainer
 
 FLAGS = flags.FLAGS
@@ -49,7 +55,7 @@ flags.DEFINE_string('model_args', None, 'JSON of the model arguments: depth, fov
 flags.DEFINE_string('train_dir', '/tmp', 'Where checkpoints are written.')
 flags.DEFINE_integer('batch_size', 4, 'Number of images in a batch.')
 flags.DEFINE_integer('max_steps', 10000, 'Number of steps to train for.')
-flags.DEFINE_integer('summary_rate_secs', 120, 'How often to log the loss, in seconds.')
+flags.DEFINE_integer('summary_rate_secs', 120, 'How often to log the loss and write summaries, in seconds.')
 flags.DEFINE_float('seed_pad', 0.05, 'Value to use for the unknown area of the seed.')
 flags.DEFINE_float('threshold', 0.9, 'Value to be reached or exceeded at the new center of the field of view in '
                    'order for the network to move.')
@@ -178,24 +184,47 @@ def main(argv):
                         FLAGS.fov_policy, FLAGS.fov_moves, FLAGS.seed_pad, FLAGS.threshold, shifts, offset_scale,
                         FLAGS.image_mean, FLAGS.image_stddev)
   os.makedirs(FLAGS.train_dir, exist_ok=True)
-  losses = []
-  t_log = t_ckpt = time.time()
-  step = 0
-  while step < FLAGS.max_steps:
-    n = min(STEPS_PER_CALL, FLAGS.max_steps - step)
-    losses.extend(trainer.train(loop, n).tolist())
-    step += n
-    now = time.time()
-    if now - t_log > FLAGS.summary_rate_secs:
-      logging.info('step %d: loss %.6f (mean of the last %d steps)', step, np.mean(losses[-n:]), n)
-      t_log = now
-    if now - t_ckpt > FLAGS.checkpoint_secs:
-      save_checkpoint(FLAGS.train_dir, trainer)
-      t_ckpt = now
-  save_checkpoint(FLAGS.train_dir, trainer)
+  losses = run(trainer, loop, order, FLAGS.train_dir, FLAGS.max_steps, FLAGS.summary_rate_secs, FLAGS.checkpoint_secs)
   np.save(os.path.join(FLAGS.train_dir, 'losses.npy'), np.array(losses))
   loop.close()
   trainer.close()
+
+
+def write_summaries(writer, trainer, loop, volume_names, step, loss):
+  """Reads and resets the tracker, and appends its summaries with the model's scalars as one event at `step`."""
+  values = tracker.summaries(loop.tracker(reset=True), volume_names)
+  values += [('pixel_loss', loss), ('optimizer_loss', loss), ('learning_rate', float(trainer.current_learning_rate()))]
+  writer.add(step, values)
+  v = dict(values)
+  if v.get('eval/patches'):
+    logging.info('step %d: eval/patch_loss %.4f, eval/all/f1 %.4f, eval/all/accuracy %.4f, moves/all/correct %.4f '
+                 '(%d patches)', step, v['eval/patch_loss'], v['eval/all/f1'], v['eval/all/accuracy'],
+                 v['moves/all/correct'], v['eval/patches'])
+
+
+def run(trainer, loop, volume_names, train_dir, max_steps, summary_rate_secs, checkpoint_secs, clock=time.time):
+  """Trains max_steps steps in calls of STEPS_PER_CALL; at the first call boundary after summary_rate_secs the
+  loss is logged and the summaries written, after checkpoint_secs a checkpoint, and one at the end.  Returns the
+  losses."""
+  writer = summary.EventWriter(train_dir)
+  losses = []
+  t_log = t_ckpt = clock()
+  step = 0
+  while step < max_steps:
+    n = min(STEPS_PER_CALL, max_steps - step)
+    losses.extend(trainer.train(loop, n).tolist())
+    step += n
+    now = clock()
+    if now - t_log > summary_rate_secs:
+      logging.info('step %d: loss %.6f (mean of the last %d steps)', step, np.mean(losses[-n:]), n)
+      write_summaries(writer, trainer, loop, volume_names, step, losses[-1])
+      t_log = now
+    if now - t_ckpt > checkpoint_secs:
+      save_checkpoint(train_dir, trainer)
+      t_ckpt = now
+  save_checkpoint(train_dir, trainer)
+  writer.close()
+  return losses
 
 
 if __name__ == '__main__':
