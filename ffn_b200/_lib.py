@@ -39,6 +39,7 @@ EXPORTS = [
     'ffn_partition_rows', 'ffn_coordinate_records', 'ffn_clean_up', 'ffn_trainer_create', 'ffn_trainer_destroy',
     'ffn_trainer_step', 'ffn_trainer_gradients', 'ffn_trainer_get_weights', 'ffn_trainer_train', 'ffn_examples_create',
     'ffn_examples_destroy', 'ffn_examples_next', 'ffn_examples_update', 'ffn_examples_read_seeds', 'ffn_examples_tracker',
+    'ffn_trainer_get_state', 'ffn_trainer_set_state', 'ffn_examples_get_state', 'ffn_examples_set_state',
     'ffn_selftest_wgmma',
 ]
 
@@ -252,6 +253,9 @@ def load() -> C.CDLL:
   lib.ffn_examples_update.argtypes = [p, p]
   lib.ffn_examples_read_seeds.argtypes = [p, p]
   lib.ffn_examples_tracker.argtypes = [p, C.POINTER(TrackerCounts), p, C.c_int, p, p, C.POINTER(C.c_int32), C.c_int]
+  for obj in ('trainer', 'examples'):
+    getattr(lib, 'ffn_%s_get_state' % obj).argtypes = [p, p, C.c_int64, C.POINTER(C.c_int64)]
+    getattr(lib, 'ffn_%s_set_state' % obj).argtypes = [p, p, C.c_int64]
   lib.ffn_selftest_wgmma.argtypes = [C.c_int, C.POINTER(C.c_double), C.c_int]
   for name in EXPORTS:
     if name not in ('ffn_last_error', 'ffn_engine_destroy', 'ffn_canvas_destroy', 'ffn_trainer_destroy',
@@ -264,6 +268,20 @@ def load() -> C.CDLL:
 def check(rc: int):
   if rc != 0:
     raise RuntimeError(load().ffn_last_error().decode('utf-8', 'replace'))
+
+
+def get_state(fn, handle) -> np.ndarray:
+  """The state blob of ffn_trainer_get_state or ffn_examples_get_state, as uint8: sized by a first call."""
+  n = C.c_int64()
+  check(fn(handle, None, 0, C.byref(n)))
+  out = np.empty(n.value, np.uint8)
+  check(fn(handle, ptr(out), len(out), C.byref(n)))
+  return out
+
+
+def set_state(fn, handle, blob):
+  b = np.ascontiguousarray(blob, dtype=np.uint8).reshape(-1)
+  check(fn(handle, ptr(b), len(b)))
 
 
 def i3(v):

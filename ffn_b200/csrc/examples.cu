@@ -3,12 +3,14 @@
 // steps (examples_advance, examples_paste).
 
 #include <cmath>
+#include <cstring>
 #include <memory>
 #include <string>
 #include <vector>
 
 #include "example_kernels.cuh"
 #include "host.cuh"
+#include "state_blob.cuh"
 
 using namespace ffn;
 
@@ -17,6 +19,7 @@ struct FfnExamples {
   int device = 0, n_volumes = 0;
   exk::Args a{};
   std::vector<FfnExampleVolume> vols;   // shapes only (the host pointers are not kept)
+  std::vector<int> shifts;              // the fixed policy's shifts, [n_shifts][3]
   FfnExampleDesc desc{};
   int64_t coords_cap = 0;
   FfnExampleCoord* coords = nullptr;
@@ -36,11 +39,12 @@ namespace {
 int grid_blocks(long long n) { return (int)std::min<long long>((n + exk::kThreads - 1) / exk::kThreads, 128); }
 
 // Every entry must name a volume, crop inside it, and permute and reflect only the axes the description allows.
-int check_coords(const FfnExamples* ex, const FfnExampleCoord* coords, int64_t n) {
+// Messages name entry i as `what` i.
+int check_coords(const FfnExamples* ex, const FfnExampleCoord* coords, int64_t n, const char* what = "stream entry ") {
   const exk::Args& a = ex->a;
   for (int64_t i = 0; i < n; ++i) {
     const FfnExampleCoord& c = coords[i];
-    const std::string at = "stream entry " + std::to_string(i) + ": ";
+    const std::string at = what + std::to_string(i) + ": ";
     if (c.volume < 0 || c.volume >= ex->n_volumes) return fail(at + "unknown volume " + std::to_string(c.volume));
     const FfnExampleVolume& v = ex->vols[c.volume];
     int seen = 0;
@@ -56,6 +60,106 @@ int check_coords(const FfnExamples* ex, const FfnExampleCoord* coords, int64_t n
       if (p != d && !(ex->desc.permutable_zyx[d] && ex->desc.permutable_zyx[p]))
         return fail(at + "permutes an axis that is not permutable");
       if (c.reflect_zyx[d] && !ex->desc.reflectable_zyx[d]) return fail(at + "reflects an axis that is not reflectable");
+    }
+  }
+  return 0;
+}
+
+// The loop's state blob.  The header holds everything the payload's meaning depends on; the payload is the per-element
+// device state in the order of state_sections.  Per-step scratch (used, entry, tk_part, tk_arrived, tk_slot, the
+// staging buffers and the uploaded coords) is rewritten by every step before it is read, and is not saved.
+constexpr uint64_t kStateMagic = 0x31545358454E4646ull;   // "FFNEXST1", little-endian
+constexpr uint32_t kStateVersion = 1;
+
+blob::Header state_header(const FfnExamples* ex) {
+  const exk::Args& a = ex->a;
+  blob::Header h;
+  h.add("policy", a.policy);
+  h.add3("field of view", a.F);
+  h.add3("deltas", a.D);
+  h.add("moves", a.moves);
+  h.add3("patch extent", a.S);
+  h.add("batch", a.batch);
+  h.add("qcap", a.qcap);
+  h.add("side", a.side);
+  h.add("n_radii", ex->n_radii);
+  h.add("number of shifts", a.n_shifts);
+  for (int i = 0; i < a.n_shifts; ++i) h.add3("shift list", ex->shifts.data() + 3 * i);
+  h.add_bits("seed threshold", a.seed_thr);
+  h.add_bits("label threshold", a.label_thr);
+  h.add_bits("eval threshold", a.eval_thr);
+  h.add_bits("pad logit", a.pad_logit);
+  h.add_bits("centre logit", a.centre_logit);
+  h.add3("permutable axes", ex->desc.permutable_zyx);
+  h.add3("reflectable axes", ex->desc.reflectable_zyx);
+  h.add("number of volumes", ex->n_volumes);
+  for (int i = 0; i < ex->n_volumes; ++i) {
+    const FfnExampleVolume& v = ex->vols[i];
+    const std::string n = "volume " + std::to_string(i);
+    h.add3(n + " image shape", v.image_shape_zyx);
+    h.add3(n + " label shape", v.label_shape_zyx);
+    h.add_bits(n + " offset", v.offset);
+    h.add_bits(n + " scale", v.scale);
+  }
+  return h;
+}
+
+std::vector<blob::Section> state_sections(const FfnExamples* ex) {
+  const exk::Args& a = ex->a;
+  const size_t B = a.batch, patch = B * a.SV * 4;
+  const size_t tk = (exk::kTkMoves + 3 * ex->n_radii) * sizeof(long long);
+  const size_t queue = B * a.qcap * 3 * sizeof(int), done = B * a.side * a.side * a.side;
+  const size_t ring = exk::kRing * (size_t)exk::plane_floats(a.E) * 4;
+  return {{a.st, B * sizeof(exk::State), false},
+          {a.ecoord, B * sizeof(FfnExampleCoord), false},
+          {a.total, sizeof(long long), false},
+          {a.tk, tk, false},
+          {a.tk_loss, sizeof(double), false},
+          {a.queue, queue, false},
+          {a.done, done, false},
+          {a.seed, patch, false},
+          {a.image, patch, false},
+          {a.labels, patch, false},
+          {a.ring, ring, false},
+          {a.ring_coord, exk::kRing * sizeof(FfnExampleCoord), false}};
+}
+
+// The checks of a payload that has passed blob::open: every value a kernel uses as an index or a bound lies in range.
+int check_state(const FfnExamples* ex, const uint8_t* payload, const std::vector<blob::Section>& secs) {
+  const exk::Args& a = ex->a;
+  std::vector<exk::State> st(a.batch);
+  std::vector<FfnExampleCoord> ec(a.batch);
+  long long total = 0;
+  std::vector<long long> tk(secs[3].bytes / sizeof(long long));
+  std::memcpy(st.data(), payload + blob::offset(secs, 0), secs[0].bytes);
+  std::memcpy(ec.data(), payload + blob::offset(secs, 1), secs[1].bytes);
+  std::memcpy(&total, payload + blob::offset(secs, 2), sizeof(long long));
+  std::memcpy(tk.data(), payload + blob::offset(secs, 3), secs[3].bytes);
+  if (total < 0) return fail("example loop state with a negative example count");
+  for (size_t i = 0; i < tk.size(); ++i)
+    if (tk[i] < 0) return fail("example loop state with a negative tracker counter");
+  const int* queue = reinterpret_cast<const int*>(payload + blob::offset(secs, 5));
+  for (int e = 0; e < a.batch; ++e) {
+    const exk::State& s = st[e];
+    const std::string at = "example loop state, element " + std::to_string(e) + ": ";
+    if (s.active != 0 && s.active != 1) return fail(at + "active is neither 0 nor 1");
+    // fixed resumes at shift k - 1 (0: the centre); k = n_shifts + 1 once the last shift was yielded or exhausted
+    if (s.k < 0 || s.k > a.n_shifts + 1)
+      return fail(at + "k = " + std::to_string(s.k) + " outside [0, " + std::to_string(a.n_shifts + 1) + "]");
+    if (s.head < 0 || s.head > s.tail || s.tail > a.qcap)
+      return fail(at + "queue head " + std::to_string(s.head) + " and tail " + std::to_string(s.tail) +
+                  " outside 0 <= head <= tail <= " + std::to_string(a.qcap));
+    for (int d = 0; d < 3; ++d)
+      if (std::abs(s.off[d]) > a.D[d] * a.moves) return fail(at + "offset outside deltas * moves");
+    // a queued offset is a yielded offset plus a face voxel at most deltas away
+    for (int j = 0; j < s.tail; ++j)
+      for (int d = 0; d < 3; ++d)
+        if (std::abs(queue[((size_t)e * a.qcap + j) * 3 + d]) > a.D[d] * (a.moves + 1))
+          return fail(at + "queued offset outside deltas * (moves + 1)");
+    if (s.active) {
+      if (s.example < 0 || s.example >= total) return fail(at + "example index outside the examples loaded");
+      const std::string what = "example loop state, the example of element " + std::to_string(e) + ": entry ";
+      if (check_coords(ex, &ec[e], 1, what.c_str())) return 1;
     }
   }
   return 0;
@@ -203,6 +307,7 @@ int ffn_examples_create(int device, const FfnModelDesc* model, const FfnExampleD
   }
   ex->desc = *desc;
   ex->desc.shifts_zyx = nullptr;
+  if (a.n_shifts) ex->shifts.assign(desc->shifts_zyx, desc->shifts_zyx + a.n_shifts * 3);
   ex->n_volumes = n_volumes;
 
   cudaDeviceProp prop{};
@@ -346,6 +451,25 @@ int ffn_examples_tracker(FfnExamples* ex, FfnTrackerCounts* out, int64_t* moves_
   for (int r = 0; r < n_radii; ++r)
     for (int t = 0; t < 3; ++t) moves_by_radius[r * 3 + t] = r < ex->n_radii ? tk[exk::kTkMoves + r * 3 + t] : 0;
   *n_planes = n;
+  return 0;
+}
+
+int ffn_examples_get_state(FfnExamples* ex, void* out, int64_t cap, int64_t* n) {
+  if (!ex) return fail("null examples");
+  CUDA_OK(cudaSetDevice(ex->device));
+  return blob::get(kStateMagic, kStateVersion, state_header(ex), state_sections(ex), out, cap, n);
+}
+
+int ffn_examples_set_state(FfnExamples* ex, const void* state, int64_t n) {
+  if (!ex) return fail("null examples");
+  const std::vector<blob::Section> secs = state_sections(ex);
+  const uint8_t* payload = nullptr;
+  if (blob::open(state, n, kStateMagic, kStateVersion, state_header(ex), secs, "example loop", &payload) ||
+      check_state(ex, payload, secs))
+    return 1;
+  CUDA_OK(cudaSetDevice(ex->device));
+  if (blob::put(payload, secs)) return 1;
+  std::memcpy(&ex->total, payload + blob::offset(secs, 2), sizeof(long long));
   return 0;
 }
 

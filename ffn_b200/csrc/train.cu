@@ -9,6 +9,7 @@
 
 #include "device_types.cuh"
 #include "host.cuh"
+#include "state_blob.cuh"
 #include "train_kernels.cuh"
 
 using namespace ffn;
@@ -222,6 +223,29 @@ int copy_params(const FfnTrainer* t, const float* src, float* const* w, float* c
   return 0;
 }
 
+// The trainer's state blob: the header names what the payload's layout depends on; the payload is the step count and
+// Adam's beta powers, then params, slot_a and slot_b in the device layout (w_off / b_off).
+constexpr uint64_t kStateMagic = 0x31545352544E4646ull;   // "FFNTRST1", little-endian
+constexpr uint32_t kStateVersion = 1;
+
+struct Scalars {
+  int64_t global_step;
+  float beta1_power, beta2_power;
+};
+
+blob::Header state_header(const FfnTrainer* t) {
+  blob::Header h;
+  h.add("depth", t->nconv / 2);
+  h.add("optimizer", t->desc.optimizer);
+  h.add("nparam", t->nparam);
+  return h;
+}
+
+std::vector<blob::Section> state_sections(FfnTrainer* t, Scalars* sc) {
+  const size_t pb = (size_t)t->nparam * 4;
+  return {{sc, sizeof(Scalars), true}, {t->params, pb, false}, {t->slot_a, pb, false}, {t->slot_b, pb, false}};
+}
+
 }  // namespace
 
 extern "C" {
@@ -382,6 +406,33 @@ int ffn_trainer_get_weights(FfnTrainer* t, float* const* weights_dhwio, float* c
   CUDA_OK(cudaSetDevice(t->device));
   if (global_step) *global_step = t->global_step;
   return copy_params(t, t->params, weights_dhwio, biases);
+}
+
+}  // extern "C"
+
+extern "C" {
+
+int ffn_trainer_get_state(FfnTrainer* t, void* out, int64_t cap, int64_t* n) {
+  if (!t) return fail("null trainer");
+  CUDA_OK(cudaSetDevice(t->device));
+  Scalars sc{t->global_step, t->beta1_power, t->beta2_power};
+  return blob::get(kStateMagic, kStateVersion, state_header(t), state_sections(t, &sc), out, cap, n);
+}
+
+int ffn_trainer_set_state(FfnTrainer* t, const void* state, int64_t n) {
+  if (!t) return fail("null trainer");
+  Scalars sc{};
+  const std::vector<blob::Section> secs = state_sections(t, &sc);
+  const uint8_t* payload = nullptr;
+  if (blob::open(state, n, kStateMagic, kStateVersion, state_header(t), secs, "trainer", &payload)) return 1;
+  std::memcpy(&sc, payload, sizeof(Scalars));
+  if (sc.global_step < 0) return fail("trainer state with a negative global step");
+  CUDA_OK(cudaSetDevice(t->device));
+  if (blob::put(payload, secs)) return 1;
+  t->global_step = sc.global_step;
+  t->beta1_power = sc.beta1_power;
+  t->beta2_power = sc.beta2_power;
+  return 0;
 }
 
 }  // extern "C"

@@ -91,6 +91,28 @@ class ExampleStream:
       out[i] = (self.volume_index[r], self.centers_xyz[r], perm, refl)
     return out
 
+  def get_state(self) -> dict:
+    """The position in the stream: the generator's MT19937 state, this epoch's order and the position in it, as
+    numpy values."""
+    _, keys, pos, has_gauss, gauss = self.rng.get_state()
+    return {'rng_keys': np.array(keys, np.uint32), 'rng_pos': np.int64(pos), 'rng_has_gauss': np.int64(has_gauss),
+            'rng_gauss': np.float64(gauss), 'order': self._order.copy(), 'pos': np.int64(self._pos)}
+
+  def set_state(self, state: Mapping[str, np.ndarray]):
+    """Continues the stream where `get_state` left it.  A state that does not fit this stream's records is refused
+    (ValueError), changing nothing."""
+    n = len(self.centers_xyz)
+    order = np.asarray(state['order'], np.int64).reshape(-1)
+    pos = int(state['pos'])
+    if len(order) not in (0, n) or (len(order) and not np.array_equal(np.sort(order), np.arange(n))):
+      raise ValueError('the stream state\'s epoch order is not a permutation of this stream\'s %d records' % n)
+    if not 0 <= pos <= len(order):
+      raise ValueError('the stream state\'s position %d lies outside its epoch of %d records' % (pos, len(order)))
+    rng = np.random.RandomState()
+    rng.set_state(('MT19937', np.asarray(state['rng_keys'], np.uint32), int(state['rng_pos']),
+                   int(state['rng_has_gauss']), float(state['rng_gauss'])))
+    self.rng, self._order, self._pos = rng, order, pos
+
 
 def _image_volume(v, name):
   v = np.asarray(v)
@@ -206,6 +228,23 @@ class ExampleLoop:
   def consume(self, n: int):
     self._pending = self._pending[n:]
     self.consumed += n
+
+  def get_state(self) -> dict:
+    """The loop's state: the device blob (ffn_examples_get_state: per element the patches, the seed, the move policy
+    and the tracker), the stream entries drawn but not yet consumed and the count consumed.  Reads only; it may be
+    taken between `next` and `update`.  The stream's own state is `stream.get_state()`."""
+    return {'device': _lib.get_state(self._lib.ffn_examples_get_state, self.handle), 'pending': self._pending.copy(),
+            'consumed': np.int64(self.consumed)}
+
+  def set_state(self, state: Mapping[str, np.ndarray]):
+    """Restores a `get_state` of a loop of the same geometry, thresholds, shifts and volumes.  A refused state
+    (RuntimeError names the field that differs) changes nothing."""
+    pending = np.asarray(state['pending'])
+    if pending.dtype != _lib.EXAMPLE_COORD_DTYPE or pending.ndim != 1:
+      raise ValueError('the loop state\'s pending entries are not a 1-d array of stream entries')
+    _lib.set_state(self._lib.ffn_examples_set_state, self.handle, state['device'])
+    self._pending = pending.copy()
+    self.consumed = int(state['consumed'])
 
   def next(self):
     """One step of the loop: (seed, image, labels) [batch, Z, Y, X] float32, offsets [batch, 3] (z, y, x) from the

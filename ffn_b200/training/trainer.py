@@ -149,6 +149,16 @@ class Trainer:
     loop.consume(int(n.value))
     return losses
 
+  def get_state(self) -> np.ndarray:
+    """Everything a later step depends on, as a uint8 blob: the global step, Adam's beta powers, the weights and the
+    optimizer slots (ffn_trainer_get_state).  Reads only."""
+    return _lib.get_state(self._lib.ffn_trainer_get_state, self._h)
+
+  def set_state(self, blob):
+    """Restores a `get_state` blob of a trainer of the same depth and optimizer.  The hyperparameters stay this
+    trainer's own.  A refused blob (RuntimeError) changes nothing."""
+    _lib.set_state(self._lib.ffn_trainer_set_state, self._h, blob)
+
   def weights(self):
     """(weights, biases) in the layout `Engine` and ffn_b200/tf_checkpoint.py use."""
     ws = [np.empty(sh, np.float32) for sh in self.shapes[0]]

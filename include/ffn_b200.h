@@ -564,6 +564,30 @@ int ffn_examples_tracker(FfnExamples* examples, FfnTrackerCounts* out, int64_t* 
 int ffn_trainer_train(FfnTrainer* trainer, FfnExamples* examples, const FfnExampleCoord* coords, int64_t n_coords,
                       int n_steps, const float* learning_rate, double* losses_out, int64_t* n_consumed);
 
+/* ---- training state: tf.train.MonitoredTrainingSession with its Saver (train.py:326-335) -----------------------
+ * Opaque, versioned blobs of everything a trainer or an example loop carries from one step to the next, so that a
+ * restored object continues bit for bit as the saved one would have.  A blob is a 32-byte prefix (uint64 magic,
+ * uint32 version, uint32 number of header words, uint64 payload bytes, uint64 FNV-1a 64 checksum of all that follows
+ * the prefix), int64 header words, then the payload.
+ *   trainer: header (depth, optimizer, nparam); payload int64 global_step, float32 beta1_power, beta2_power, then
+ *     params, slot_a and slot_b (float32 [nparam] each, in the device layout).  The hyperparameters (momentum, betas,
+ *     epsilon, clip) are the restoring trainer's own.
+ *   example loop: header (policy, fov, deltas, moves, patch extent, batch, qcap, side, n_radii, the shift list, the
+ *     seed, label and eval thresholds and the pad and centre logits bit for bit, the permutable and reflectable axes,
+ *     and every volume's shapes, offset and scale); payload per element the policy state, the current example's
+ *     stream entry, the example count, the tracker's counters, loss and ring, the max_pred_moves queues and visited
+ *     cells, and the seed, image and label patches.
+ * get_state: *n = the blob's size; the blob is written only when out is not NULL and cap >= *n (call again with
+ * cap = *n).  It only reads: saving changes nothing later.  It may be called between ffn_examples_next and
+ * ffn_examples_update (the paste uses the saved offsets).
+ * set_state: checks the whole blob on the host first — length, magic, version, checksum, every header word (a
+ * difference is refused with the field's name) and every saved index or bound (policy state, queued offsets, each
+ * example's stream entry) — and changes nothing when it refuses. */
+int ffn_trainer_get_state(FfnTrainer* trainer, void* out, int64_t cap, int64_t* n);
+int ffn_trainer_set_state(FfnTrainer* trainer, const void* state, int64_t n);
+int ffn_examples_get_state(FfnExamples* examples, void* out, int64_t cap, int64_t* n);
+int ffn_examples_set_state(FfnExamples* examples, const void* state, int64_t n);
+
 /* Known-answer test of the wgmma descriptors (worst absolute error of each case in out[]; see
  * ffn_selftest_wgmma in ffn_b200/csrc/engine.cu).  Used by tests, not by the product path. */
 int ffn_selftest_wgmma(int device, double* out, int n_out);

@@ -18,7 +18,19 @@ ffn_b200.training.trainer).  Differences from the reference script:
   * weights start as tf_slim does (glorot-uniform weights, zero biases), drawn from `--seed` (with a generator of its
     own, so the weights are not correlated with the data order);
   * checkpoints are `model.ckpt-<step>.npz` files of w00.. / b00.. arrays (what ffn_b200/tf_checkpoint.py and
-    run_inference.py read), written every 300 s and at the end; a run does not resume from them;
+    run_inference.py read), written every `--checkpoint_secs` and at the end.  Each is followed by
+    `train_state-<step>.npz` (the newest 5 are kept): the weights with the optimizer slots and Adam's beta powers, the
+    device example loop (every element's patches, seed, move policy and tracker), the position in the example stream,
+    the losses so far and the flags that define the run;
+  * a run resumes, as MonitoredTrainingSession does: when `--train_dir` holds a training state, the newest one is
+    restored before the first step and the run continues bit for bit as if it had not stopped.  The flags that
+    define the run (the model, batch, policy, seed, thresholds, axes, optimizer, normalisation, volumes and the number
+    of coordinate records) must be those of the saved run, or it is refused before any device work; the learning rate
+    and its decay, momentum, the betas, epsilon, the clip, `--max_steps` and the summary and checkpoint intervals may
+    change.  A run whose `--max_steps` is already reached exits without writing;
+  * `--init_checkpoint` starts a fresh run from saved weights (an .npz of w00.. / b00.. arrays or a TF1 checkpoint
+    prefix such as the published FIB-25 model) at step 0 with zero optimizer slots, as the JAX trainer's
+    init_from_cpoint does; it is ignored when there is a state to resume from;
   * every `--summary_rate_secs`, at the first boundary of a call of STEPS_PER_CALL steps after that time, the loss
     is logged and the EvalTracker summaries (moves, the final object masks' loss and prediction metrics, their
     centre slices; ffn_b200.training.tracker), with pixel_loss, optimizer_loss and learning_rate, are appended to a
@@ -33,12 +45,14 @@ import json
 import logging
 import os
 import random
+import re
 import time
 
 import numpy as np
 from absl import app
 from absl import flags
 
+from ffn_b200 import tf_checkpoint
 from ffn_b200.training import examples as ex
 from ffn_b200.training import inputs
 from ffn_b200.training import summary
@@ -82,8 +96,15 @@ flags.DEFINE_float('max_gradient_entry_mag', 0.7, 'Clip every gradient entry to 
 flags.DEFINE_integer('seed', 0, 'Seed of the weights, the example stream with its augmentation, and the move order '
                      '(each from its own generator, derived from this seed).')
 flags.DEFINE_integer('checkpoint_secs', 300, 'How often to write a checkpoint, in seconds.')
+flags.DEFINE_string('init_checkpoint', None, 'Weights to start a fresh run from instead of the glorot initialisation: '
+                    'an .npz of w00.. / b00.. arrays or a TF1 checkpoint prefix (model.ckpt-N).  Ignored when '
+                    '--train_dir holds a training state to resume from.')
 
 STEPS_PER_CALL = 50
+STATES_KEPT = 5   # the reference's tf.train.Saver keeps its default max_to_keep=5
+STATE_FILE = re.compile(r'^train_state-(\d+)\.npz$')
+# fingerprint entries that are not a flag of their own, and the flags they come from
+_FINGERPRINT_FLAGS = {'volumes': '--data_volumes / --label_volumes', 'coordinate_records': '--train_coords'}
 
 
 def read_volume(spec):
@@ -149,6 +170,89 @@ def save_checkpoint(train_dir, trainer):
   return path
 
 
+def load_init_checkpoint(path, depth):
+  """(weights, biases) of --init_checkpoint: an .npz of w00.. / b00.. arrays, or else a TF1 checkpoint prefix (chosen
+  by suffix, as the inference executor chooses).  A network of another depth is refused: reading the first layers of
+  a deeper TF checkpoint would silently truncate it."""
+  if path.endswith('.npz'):
+    with np.load(path) as z:
+      n = len([k for k in z.files if k.startswith('w')])
+    if n != 2 * depth + 1:
+      raise ValueError('--init_checkpoint %s holds %d weight arrays; a network of depth %d (--model_args) has %d' %
+                       (path, n, depth, 2 * depth + 1))
+    return tf_checkpoint.load_convstack_npz(path)
+  names = tf_checkpoint.list_variables(path)
+  deeper = 'seed_update/conv%d_a/weights' % depth in names
+  if deeper or 'seed_update/conv%d_b/weights' % (depth - 1) not in names:
+    raise ValueError('--init_checkpoint %s is not a network of depth %d (--model_args): it %s' %
+                     (path, depth, 'has more residual modules' if deeper else 'has fewer residual modules'))
+  return tf_checkpoint.load_convstack_weights(path, depth)
+
+
+def run_fingerprint(model, images, labels, n_records):
+  """The flags and data that define what a run's steps mean.  A resumed run must have the saved run's."""
+  return {
+      'model_args': model, 'batch_size': FLAGS.batch_size, 'fov_policy': FLAGS.fov_policy,
+      'fov_moves': FLAGS.fov_moves, 'shuffle_moves': FLAGS.shuffle_moves, 'seed': FLAGS.seed,
+      'seed_pad': FLAGS.seed_pad, 'threshold': FLAGS.threshold,
+      'permutable_axes': sorted(int(a) for a in FLAGS.permutable_axes),
+      'reflectable_axes': sorted(int(a) for a in FLAGS.reflectable_axes), 'optimizer': FLAGS.optimizer,
+      'image_mean': FLAGS.image_mean, 'image_stddev': FLAGS.image_stddev,
+      'image_offset_scale_map': FLAGS.image_offset_scale_map or [],
+      'volumes': {n: [list(images[n].shape), list(labels[n].shape)] for n in sorted(images)},
+      'coordinate_records': n_records,
+  }
+
+
+def newest_state(train_dir):
+  """The path of the training state of the highest step in train_dir, or None."""
+  if not os.path.isdir(train_dir):
+    return None
+  steps = [int(m.group(1)) for m in map(STATE_FILE.match, os.listdir(train_dir)) if m]
+  return os.path.join(train_dir, 'train_state-%d.npz' % max(steps)) if steps else None
+
+
+def load_state(path, fingerprint):
+  """The arrays of a training state, after its run fingerprint was found equal to this run's (ValueError naming the
+  first flag that differs)."""
+  with np.load(path) as z:
+    state = {k: z[k] for k in z.files}
+  saved = json.loads(str(state['fingerprint']))
+  for key in sorted(set(saved) | set(fingerprint)):
+    if saved.get(key) != fingerprint.get(key):
+      raise ValueError('%s differs from the run saved in %s (saved %r, given %r): a run resumes only with the flags '
+                       'that define it; use another --train_dir for a new run' %
+                       (_FINGERPRINT_FLAGS.get(key, '--' + key), path, saved.get(key), fingerprint.get(key)))
+  return state
+
+
+def save_state(train_dir, trainer, loop, losses, fingerprint, keep=STATES_KEPT):
+  """Writes train_state-<step>.npz atomically (a temporary file renamed over it) and deletes all but the newest
+  `keep` state files."""
+  step = trainer.global_step
+  path = os.path.join(train_dir, 'train_state-%d.npz' % step)
+  tmp = path + '.tmp.npz'
+  ls = loop.get_state()
+  np.savez(tmp, fingerprint=np.array(json.dumps(fingerprint, sort_keys=True)), step=np.int64(step),
+           trainer=trainer.get_state(), loop_device=ls['device'], loop_pending=ls['pending'],
+           loop_consumed=ls['consumed'], losses=np.asarray(losses, np.float64),
+           **{'stream_' + k: v for k, v in loop.stream.get_state().items()})
+  os.replace(tmp, path)
+  steps = sorted(int(m.group(1)) for m in map(STATE_FILE.match, os.listdir(train_dir)) if m)
+  for old in steps[:-keep]:
+    os.remove(os.path.join(train_dir, 'train_state-%d.npz' % old))
+  return path
+
+
+def restore_state(state, trainer, loop):
+  """Restores a load_state result into a trainer and a loop; returns the losses of the steps run so far."""
+  trainer.set_state(state['trainer'])
+  loop.stream.set_state({k[len('stream_'):]: v for k, v in state.items() if k.startswith('stream_')})
+  loop.set_state({'device': state['loop_device'], 'pending': state['loop_pending'],
+                  'consumed': state['loop_consumed']})
+  return state['losses'].tolist()
+
+
 def main(argv):
   del argv
   if not FLAGS.model_name.endswith('ConvStack3DFFNModel'):
@@ -169,6 +273,21 @@ def main(argv):
   labels = parse_volumes(FLAGS.label_volumes)
   centers, names = inputs.load_coordinates(FLAGS.train_coords)
   order, vol_index = volume_indices(names, images, labels)
+  model = {'depth': depth, 'fov_size': list(fov_zyx[::-1]), 'deltas': list(deltas_zyx[::-1])}
+  fingerprint = run_fingerprint(model, {n: images[n] for n in order}, {n: labels[n] for n in order}, len(centers))
+  state_path = newest_state(FLAGS.train_dir)
+  state = load_state(state_path, fingerprint) if state_path else None
+  if state is not None:
+    if FLAGS.init_checkpoint:
+      logging.info('--init_checkpoint %s ignored: resuming from %s', FLAGS.init_checkpoint, state_path)
+    if FLAGS.max_steps <= int(state['step']):
+      logging.info('%s is at step %d, --max_steps is %d: nothing to train', state_path, int(state['step']),
+                   FLAGS.max_steps)
+      return
+  elif os.path.isdir(FLAGS.train_dir) and any(f.startswith('model.ckpt-') for f in os.listdir(FLAGS.train_dir)):
+    logging.warning('%s holds weight checkpoints but no training state: starting a fresh run at step 0 (to start from '
+                    'saved weights, pass one of them as --init_checkpoint)', FLAGS.train_dir)
+  init = load_init_checkpoint(FLAGS.init_checkpoint, depth) if FLAGS.init_checkpoint and state is None else None
   # separate generators for the stream, the weights and the move order, so that none reuses another's draws
   stream_seed, weight_seed, move_seed = (int(s.generate_state(1)[0])
                                          for s in np.random.SeedSequence(FLAGS.seed).spawn(3))
@@ -178,13 +297,21 @@ def main(argv):
   shifts = ex.model_shifts(deltas_zyx)
   if FLAGS.shuffle_moves:
     random.Random(move_seed).shuffle(shifts)
-  ws, bs = glorot_init(depth, rng)
+  ws, bs = glorot_init(depth, rng) if init is None else init
   trainer = Trainer(ws, bs, fov_zyx, batch_size=FLAGS.batch_size, **trainer_options())
   loop = ex.ExampleLoop({n: (images[n], labels[n]) for n in order}, stream, fov_zyx, deltas_zyx, FLAGS.batch_size,
                         FLAGS.fov_policy, FLAGS.fov_moves, FLAGS.seed_pad, FLAGS.threshold, shifts, offset_scale,
                         FLAGS.image_mean, FLAGS.image_stddev)
+  losses = []
+  if state is not None:
+    losses = restore_state(state, trainer, loop)
+    logging.info('Resuming from step %d (%s)', trainer.global_step, state_path)
+  elif init is not None:
+    logging.info('Starting from the weights of %s', FLAGS.init_checkpoint)
   os.makedirs(FLAGS.train_dir, exist_ok=True)
-  losses = run(trainer, loop, order, FLAGS.train_dir, FLAGS.max_steps, FLAGS.summary_rate_secs, FLAGS.checkpoint_secs)
+  save = lambda ls: save_state(FLAGS.train_dir, trainer, loop, ls, fingerprint)
+  losses = run(trainer, loop, order, FLAGS.train_dir, FLAGS.max_steps, FLAGS.summary_rate_secs, FLAGS.checkpoint_secs,
+               losses=losses, on_checkpoint=save)
   np.save(os.path.join(FLAGS.train_dir, 'losses.npy'), np.array(losses))
   loop.close()
   trainer.close()
@@ -202,14 +329,16 @@ def write_summaries(writer, trainer, loop, volume_names, step, loss):
                  v['moves/all/correct'], v['eval/patches'])
 
 
-def run(trainer, loop, volume_names, train_dir, max_steps, summary_rate_secs, checkpoint_secs, clock=time.time):
-  """Trains max_steps steps in calls of STEPS_PER_CALL; at the first call boundary after summary_rate_secs the
-  loss is logged and the summaries written, after checkpoint_secs a checkpoint, and one at the end.  Returns the
-  losses."""
+def run(trainer, loop, volume_names, train_dir, max_steps, summary_rate_secs, checkpoint_secs, clock=time.time,
+        losses=(), on_checkpoint=None):
+  """Trains up to step max_steps in calls of STEPS_PER_CALL, from step len(losses) (the losses of the steps already
+  run); at the first call boundary after summary_rate_secs the loss is logged and the summaries written, after
+  checkpoint_secs a checkpoint, and one at the end.  on_checkpoint(losses) runs after each checkpoint.  Returns the
+  losses of every step."""
   writer = summary.EventWriter(train_dir)
-  losses = []
+  losses = list(losses)
   t_log = t_ckpt = clock()
-  step = 0
+  step = len(losses)
   while step < max_steps:
     n = min(STEPS_PER_CALL, max_steps - step)
     losses.extend(trainer.train(loop, n).tolist())
@@ -221,8 +350,12 @@ def run(trainer, loop, volume_names, train_dir, max_steps, summary_rate_secs, ch
       t_log = now
     if now - t_ckpt > checkpoint_secs:
       save_checkpoint(train_dir, trainer)
+      if on_checkpoint:
+        on_checkpoint(losses)
       t_ckpt = now
   save_checkpoint(train_dir, trainer)
+  if on_checkpoint:
+    on_checkpoint(losses)
   writer.close()
   return losses
 
